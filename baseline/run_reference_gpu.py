@@ -1,4 +1,4 @@
-"""Run the UNMODIFIED reference (pip-installed from /root/reference into baseline/_ref, git-ignored) on the GPU:
+"""Run the UNMODIFIED reference (staged under oracle/_ref by oracle/install_reference.py, git-ignored) on the GPU:
 its own LLM / flash-attn 2.8.3 / Triton / torch.compile / CUDA-graph path, on the benchmark request mix.
 
     python baseline/run_reference_gpu.py [passes]
@@ -14,7 +14,7 @@ import sys
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 def load_by_path(name, path):
@@ -27,7 +27,7 @@ def load_by_path(name, path):
 def main():
     passes = int(sys.argv[1]) if len(sys.argv) > 1 else 2
     if not os.path.isdir(os.path.join(REF, "nanovllm")):
-        print(json.dumps({"impl": "reference-gpu", "unavailable": "baseline/_ref missing (pip install --target baseline/_ref /root/reference)"}))
+        print(json.dumps({"impl": "reference-gpu", "unavailable": "oracle/_ref missing (oracle/install_reference.py)"}))
         return
     syn = load_by_path("b200_synthetic", os.path.join(ROOT, "nano-vllm_b200", "nanovllm", "utils", "synthetic.py"))
     mdir = syn.make_model_dir(os.environ.get("B200_BENCH_MODEL_DIR", "/tmp/b200_bench_models/qwen3-0.6b"), "qwen3-0.6b", seed=0)

@@ -1,13 +1,18 @@
 #!/usr/bin/env python
-"""Headline benchmark: the reference's own bench.py workload (reference bench.py:8-28) on the B200 path.
+"""Headline benchmark: the reference's own bench.py workload (reference bench.py:8-28) on this project's H100 path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one full ``LLM.generate()`` over the benchmark request mix: Qwen3-0.6B (random init, bf16),
 256 sequences, prompt and output lengths each U[100, 1024] drawn exactly like the reference
 (random.seed(0)), temperature 0.6, ignore_eos, CUDA graphs on.  Token VALUES are shifted per step so that
-no step can reuse the previous step's prefix-cache blocks (lengths, hence work, are identical).
+no step can reuse the previous step's prefix-cache blocks (lengths, hence work, are identical).  The sampler's seed is
+fixed (B200_SAMPLE_SEED, default 0), so the same arguments give the same inputs from run to run.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step's generate() returned: DIR/token_ids.npy
+(float32 [256, longest output], -1 past each sequence's end) and DIR/output_lengths.npy (float32 [256]), so that two
+builds can be compared output for output.
 
 Printed JSON (rank 0, one line):
   e2e      output tokens/s through the public API with host prompts: wall time of generate() including the
@@ -15,7 +20,7 @@ Printed JSON (rank 0, one line):
   value    the same tokens over the device-busy time only (CUDA events around each step's GPU work,
            metadata already resident in HBM): what the GPU side sustains without host overhead
   roofline paged-decode kernel: algorithmic KV bytes / CUDA-event time, sampled over the run's decode steps
-  cpu_baseline  the reference's own classes on the host CPU (oracle/ref_cpu_arm.py over baseline/_ref; the oracle port
+  cpu_baseline  the reference's own classes on the host CPU (oracle/ref_cpu_arm.py over oracle/_ref; the oracle port
            oracle/cpu_engine.py when the installed reference is absent) on a bounded sample of the same request mix
   parity   a short greedy generation OUTSIDE the timed region, checked on rank 0 against the CPU oracle (teacher-forced
            margin test) and for agreement between the tensor-parallel ranks -- the oracle is the checker here, never
@@ -30,6 +35,7 @@ import random
 import statistics
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -40,7 +46,9 @@ for _p in (ROOT, os.path.join(ROOT, "nano-vllm_b200")):
 
 METRIC = "output tokens/s, Qwen3-0.6B 256 seqs in/out 100-1024"
 README_TOK_S = 1434.13          # reference README.md:50-61, RTX 4070 Laptop (the only published number)
-MODEL_DIR = os.environ.get("B200_BENCH_MODEL_DIR", "/tmp/b200_bench_models/qwen3-0.6b")
+# the synthetic checkpoint is cached under the temporary directory, per user (the tree may be read-only)
+MODEL_DIR = os.environ.get("B200_BENCH_MODEL_DIR",
+                           os.path.join(tempfile.gettempdir(), f"b200_bench_models_{os.getuid()}", "qwen3-0.6b"))
 
 
 _T0 = time.perf_counter()
@@ -75,7 +83,7 @@ def ensure_model_dir(local_rank: int) -> str:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons while the timed region runs (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons while the timed region runs (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -117,7 +125,7 @@ def load_peaks() -> dict:
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return {"hbm_gbs": p["hbm_gbs"], "source": "MEASURED_PEAKS.json (measured copy)"}
     except Exception:
-        return {"hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+        return {"hbm_gbs": 3350.0, "source": "H100 SXM data sheet (3.35 TB/s HBM3), not a measured peak"}
 
 
 WORKLOAD = ("Qwen3-0.6B random-init bf16, 256 seqs, in/out U[100,1024] (reference bench.py shape), temperature 0.6, "
@@ -129,30 +137,9 @@ def bench_config(world: int) -> dict:
     return {"workload": WORKLOAD, "parallelism": f"tp{world}", "output_tokens_per_step": 133966}
 
 
-def ncu_traffic() -> tuple[float | None, str]:
-    """dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the decode kernel at the batch-256 step, parsed from
-    the newest committed ncu summary under profiles/ (made by profiles/summarize_ncu.py); (None, why) if absent."""
-    import glob
-    import re
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r??_decode_kernel_ncu.txt")))
-    if not files:
-        return None, "no profiles/r??_decode_kernel_ncu.txt"
-    text = open(files[-1]).read()
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    vals = {}
-    for key in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-        m = re.search(re.escape(key) + r"\s+([0-9.,]+)\s+(\w+)", text)
-        if not m or m.group(2) not in unit:
-            return None, f"{key} not found in {os.path.basename(files[-1])}"
-        vals[key] = float(m.group(1).replace(",", "")) * unit[m.group(2)]
-    rd, wr = vals["dram__bytes_read.sum"], vals["dram__bytes_write.sum"]
-    return rd + wr, (f"dram__bytes_read.sum + dram__bytes_write.sum of ONE launch at the batch-256 step, parsed from "
-                     f"profiles/{os.path.basename(files[-1])}: {rd / 1e6:.2f} MB + {wr / 1e6:.2f} MB")
-
-
 # ------------------------------------------------------------------------------------------------
 # CPU baseline -- also the --impl reference arm: the reference's own classes on host cores (oracle/ref_cpu_arm.py),
-# or the oracle port when baseline/_ref did not travel
+# or the oracle port when oracle/_ref did not travel
 # ------------------------------------------------------------------------------------------------
 CPU_SAMPLE_SEQS = 8
 
@@ -165,7 +152,7 @@ def sample_requests(step: int = 0, n: int = CPU_SAMPLE_SEQS):
 def cpu_reference_run(model_dir: str, reps: int, budget_s: float):
     """-> (list of (tokens, seconds), threads, cores, kind, description)."""
     script = os.path.join(ROOT, "oracle", "ref_cpu_arm.py")
-    have_ref = os.path.isdir(os.path.join(ROOT, "baseline", "_ref", "nanovllm"))
+    have_ref = os.path.isdir(os.path.join(ROOT, "oracle", "_ref", "nanovllm"))
     if have_ref:
         env = dict(os.environ)
         for k in ("RANK", "LOCAL_RANK", "WORLD_SIZE", "MASTER_ADDR", "MASTER_PORT", "OMP_NUM_THREADS"):
@@ -177,7 +164,7 @@ def cpu_reference_run(model_dir: str, reps: int, budget_s: float):
         if r.returncode == 0 and lines:
             d = json.loads(lines[-1])
             desc = (f"first {d['n_seqs']} requests of the benchmark mix ({d['prompt_tokens']} prompt tokens, their own output "
-                    f"lengths), temperature 0.6; the UNMODIFIED reference classes from baseline/_ref (Scheduler, BlockManager, "
+                    f"lengths), temperature 0.6; the UNMODIFIED reference classes from oracle/_ref (Scheduler, BlockManager, "
                     f"prepare_prefill/decode, Qwen3ForCausalLM, Sampler) in bf16 on CPU, attention core restated "
                     f"(flash-attn is GPU-only), torch.compile off; {d['threads']} of {d['cores']} host threads; "
                     f"each repetition stopped after {budget_s:.0f}s")
@@ -204,7 +191,7 @@ def cpu_reference_run(model_dir: str, reps: int, budget_s: float):
         produced, dt, steps = eng.generate_bounded(prompts, sps, budget_s)
         out.append((produced, dt))
         log(f"cpu sample rep {r}: {produced} tokens in {dt:.1f}s over {steps} engine steps")
-    desc = (f"first {CPU_SAMPLE_SEQS} requests of the benchmark mix; oracle PORT of the reference loop (baseline/_ref absent), "
+    desc = (f"first {CPU_SAMPLE_SEQS} requests of the benchmark mix; oracle PORT of the reference loop (oracle/_ref absent), "
             f"greedy, bf16 on CPU, {threads} of {cores} host threads; each repetition stopped after {budget_s:.0f}s")
     return out, threads, cores, "port", desc
 
@@ -301,7 +288,6 @@ def decode_roofline(llm, sample_every: int = 24, requests=None):
     achieved = tot_bytes / (tot_ms * 1e-3) / 1e9
     first = per_step[0]
     first_gbs = (first[2] * 2 * m.num_kv_heads * m.head_dim * 2) / (first[3] * 1e-6) / 1e9
-    traffic, traffic_is = ncu_traffic()
     # decode GB/s by batch-size bucket (the second half of the run lives at small batches)
     buckets = {}
     for _, n, sumctx, us in per_step:
@@ -314,13 +300,14 @@ def decode_roofline(llm, sample_every: int = 24, requests=None):
                  "frac": v[0] / (v[1] * 1e-6) / 1e9 / peaks["hbm_gbs"]} for k, v in sorted(buckets.items())]
     G = m.num_heads // m.num_kv_heads
     return {"bound": "hbm", "kernel": f"paged_decode_kernel<G={G}>" if G <= 2 else f"paged_decode_mma_kernel<G={G}>", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-            "frac": achieved / peaks["hbm_gbs"], "peak_source": peaks["source"], "frac_of_8TBs_spec": achieved / 8000.0,
-            "traffic": traffic if requests is None else None,
-            "traffic_is": (traffic_is + " (vs 587.2 MB algorithmic for that launch)") if requests is None else "not captured for this workload",
+            "frac": achieved / peaks["hbm_gbs"], "peak_source": peaks["source"], "frac_of_3_35TBs_spec": achieved / 3350.0,
+            "traffic": None,
+            "traffic_is": "DRAM counters are not read by this benchmark (they need a profiler capture of the launch); the "
+                          "figures above are algorithmic bytes over CUDA-event time",
             "launches_timed": launches, "avg_launch_us": tot_ms * 1000.0 / launches,
             "bytes_per_launch_avg": tot_bytes / launches,
             "batch256_step0": {"batch": first[1], "sum_ctx": first[2], "launch_us": first[3], "GB/s": first_gbs,
-                               "frac_measured_peak": first_gbs / peaks["hbm_gbs"], "frac_8TBs": first_gbs / 8000.0},
+                               "frac_measured_peak": first_gbs / peaks["hbm_gbs"], "frac_3_35TBs": first_gbs / 3350.0},
             "by_batch": by_batch,
             "unique_page_bytes_per_launch_avg": tot_unique / launches,
             "unique_page_GB/s": tot_unique / (tot_ms * 1e-3) / 1e9,
@@ -393,6 +380,19 @@ def parity_leg(llm, model_dir: str, world: int, rank: int) -> dict | None:
     return res
 
 
+def dump_outputs(out_dir: str, outs: list):
+    """What the last timed generate() returned, as float32 arrays (token ids < 2^24 are exact in float32)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    lens = np.asarray([len(o["token_ids"]) for o in outs], dtype=np.float32)
+    ids = np.full((len(outs), int(lens.max()) if len(outs) else 0), -1.0, dtype=np.float32)
+    for i, o in enumerate(outs):
+        ids[i, :len(o["token_ids"])] = o["token_ids"]
+    np.save(os.path.join(out_dir, "token_ids.npy"), ids)
+    np.save(os.path.join(out_dir, "output_lengths.npy"), lens)
+    log(f"outputs of the last timed step written to {out_dir}: token_ids {ids.shape}, output_lengths {lens.shape}")
+
+
 def run_b200_arm(args):
     import torch
     import torch.distributed as dist
@@ -412,6 +412,7 @@ def run_b200_arm(args):
     log("model dir ready; constructing LLM")
     from nanovllm import LLM, SamplingParams
     from nanovllm import ops
+    os.environ.setdefault("B200_SAMPLE_SEED", "0")       # same arguments, same sampled tokens
     t_init = time.perf_counter()
     llm = LLM(mdir, enforce_eager=False, max_model_len=4096, tensor_parallel_size=world)
     init_s = time.perf_counter() - t_init
@@ -419,11 +420,14 @@ def run_b200_arm(args):
     runner = llm.model_runner
     ops.reset_launch_count()
 
+    last_outs = []
+
     def one_pass(step_idx: int):
         prompts, max_tokens = bench_requests(step_idx)
         sps = [SamplingParams(temperature=0.6, ignore_eos=True, max_tokens=mt) for mt in max_tokens]
         outs = llm.generate(prompts, sps, use_tqdm=False)
         assert sum(len(o["token_ids"]) for o in outs) == sum(max_tokens)
+        last_outs[:] = outs
         return sum(max_tokens)
 
     llm.generate(["t1 t2 t3"], SamplingParams(), use_tqdm=False)          # reference bench.py:22
@@ -454,6 +458,8 @@ def run_b200_arm(args):
         wall = time.perf_counter() - t0
     ev_ms = e0.elapsed_time(e1)
     log(f"timed region: {args.steps} passes in {wall:.2f}s")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_outs)
     prof = runner.end_profile()
     ls = dict(llm.loop_stats)
     t = torch.tensor([ev_ms, prof["device_ms"]], dtype=torch.float64, device="cuda")
@@ -502,7 +508,7 @@ def run_b200_arm(args):
             "gpu_launches": prof["kernel_launches"], "clocks": clocks.summary(),
             "notes": {"value_is": "tokens / device-busy time (CUDA events around each engine step's GPU work, metadata resident)",
                       "e2e_is": "tokens / CUDA-event time around LLM.generate() with host prompts (H2D metadata + D2H tokens every engine step)",
-                      "l2": "KV read per decode step (>= 0.5 GB/layer at batch 256) and weights (1.2 GB) exceed the 126 MB L2; "
+                      "l2": "KV read per decode step (>= 0.5 GB/layer at batch 256) and weights (1.2 GB) exceed the 50 MB L2; "
                             "no flush between passes needed, token values differ per pass (no prefix-cache reuse)",
                       "vs_baseline_basis": "value (device-busy) / BASELINE.md's 1434.13 tok/s (reference README, RTX 4070 Laptop: "
                                            "the only published number, a wall-clock figure); the like-for-like wall-clock ratio is "
@@ -537,7 +543,11 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (float32 .npy files) into DIR")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference_arm(args)
     else:

@@ -1,5 +1,5 @@
 /*
- * b200_paged_attn.h -- C ABI of libb200attn.so, the B200 (sm_100a) paged-attention path that
+ * b200_paged_attn.h -- C ABI of libb200attn.so, the H100 (sm_90a) paged-attention path that
  * drops in behind nano-vLLM's attention operator and the small fused ops around it.
  *
  * Every entry point cites the reference interface (GeeeekExplorer/nano-vllm @ bb823b3e) it
@@ -46,13 +46,13 @@ enum {
     B200_ECUDA = -3,        /* a CUDA runtime call failed; b200_last_cuda_error() has the text */
     B200_ENOTBOUND = -4,    /* KV cache not bound (b200_kv_bind) */
     B200_EWORKSPACE = -5,   /* workspace too small */
-    B200_EARCH = -6         /* device is not compute capability 10.x */
+    B200_EARCH = -6         /* device is not compute capability 9.0 */
 };
 
 /* ---- lifetime ------------------------------------------------------------------------- */
 
 /* Replaces the device setup in ModelRunner.__init__ (engine/model_runner.py:26-30): selects
- * `device`, checks it is sm_100, records the SM count.  */
+ * `device`, checks it is sm_90, records the SM count.  */
 int b200_init(int device, b200_ctx** out);
 void b200_destroy(b200_ctx* ctx);
 const char* b200_strerror(int code);
@@ -211,9 +211,9 @@ int b200_sample(const void* logits, int logits_is_fp32, int64_t logits_stride0,
                 uint64_t seed, uint64_t step, const int64_t* step_dev, int64_t* out,
                 int64_t* out_keys, void* stream);
 
-/* ---- decode-size projections on tcgen05 (validated on a B200 in round 2: tests/test_gpu_linear.py) ----------------
+/* ---- decode-size projections on the tensor cores (wgmma; tests/test_gpu_linear.py) ---------------------------------
  *
- * F.linear of the reference's *ParallelLinear layers (layers/linear.py:51,73,153) for small batches, on tcgen05,
+ * F.linear of the reference's *ParallelLinear layers (layers/linear.py:51,73,153) for small batches, on wgmma,
  * with what follows fused in (csrc/linear_tc.cu):
  *   x [rows, k] bf16 (row stride x_stride0), w [n, k] bf16 contiguous, k % 64 == 0.
  *   epilogue 0: out[rows, n_out] bf16 = bf16(x w^T)                                      (k_splits must be 1)
@@ -227,8 +227,8 @@ int b200_sample(const void* logits, int logits_is_fp32, int64_t logits_stride0,
 int b200_linear(const void* x, int64_t x_stride0, const void* w, void* out, int64_t out_stride0, int rows,
                 int n_out, int k, int epilogue, int block_n, int k_splits, int flags, void* stream);
 
-/* (opt-in: parity-green, slower than the library GEMM + b200_sample) ParallelLMHead.forward + Sampler.forward in one pass (layers/embed_head.py:56-66, layers/sampler.py:7-12):
- * logits = bf16(hidden lm_head^T) are produced tile by tile in tensor memory, scored exactly as b200_sample scores
+/* (opt-in) ParallelLMHead.forward + Sampler.forward in one pass (layers/embed_head.py:56-66, layers/sampler.py:7-12):
+ * logits = bf16(hidden lm_head^T) are produced tile by tile in registers, scored exactly as b200_sample scores
  * them (same RNG keyed by (seed, step, row, vocabulary id); temperature 0 = greedy, lowest index on ties) and
  * reduced to one packed (score, token) key per row with atomicMax -- the [rows, vocab] logits are never written.
  *   hidden [rows, k] bf16 (last-token rows), lm_head [vocab, k] bf16 contiguous (this rank's shard), k % 64 == 0;

@@ -11,7 +11,7 @@ extern "C" const char* b200_strerror(int code) {
         case B200_ECUDA: return "CUDA runtime error (see b200_last_cuda_error)";
         case B200_ENOTBOUND: return "KV cache not bound (call b200_kv_bind)";
         case B200_EWORKSPACE: return "workspace too small (see b200_decode_workspace_bytes)";
-        case B200_EARCH: return "device is not compute capability 10.x (this library is sm_100a only)";
+        case B200_EARCH: return "device is not compute capability 9.0 (this library is sm_90a only)";
         default: return "unknown error";
     }
 }
@@ -22,7 +22,7 @@ extern "C" int b200_init(int device, b200_ctx** out) {
     cudaDeviceProp prop;
     cudaError_t e = cudaGetDeviceProperties(&prop, device);
     if (e != cudaSuccess) return B200_ECUDA;
-    if (prop.major != 10) return B200_EARCH;
+    if (prop.major != 9 || prop.minor != 0) return B200_EARCH;
     e = cudaSetDevice(device);
     if (e != cudaSuccess) return B200_ECUDA;
     b200_ctx* ctx = new b200_ctx();

@@ -74,9 +74,9 @@ struct B200SmemOptIn {
         e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
         // Ask for the largest shared-memory carve-out: a kernel of ANOTHER stream can only join this one on an SM if the
         // SM's current L1/shared split already has room for both (the split is not changed under a running CTA).  The
-        // two-stream decode step (models/qwen3.py::_forward_dual) relies on it: tcgen05 projections of one half batch
-        // run in the ~73 KB that the attention kernel of the other half leaves free.  A hint; none of these kernels
-        // leans on L1.
+        // two-stream decode step (models/qwen3.py::_forward_dual) relies on it: wgmma projections of one half batch
+        // run in the shared memory that the attention kernel of the other half leaves free.  A hint; none of these
+        // kernels leans on L1.
         if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         if (e == cudaSuccess) done[dev] = true;
         return e;
@@ -193,7 +193,7 @@ __device__ __forceinline__ float fast_exp2(float x) {
 // without the attribute) and every launch carries cudaLaunchAttributeProgrammaticStreamSerialization, so inside a
 // captured step the next kernel's blocks are scheduled while the previous kernel drains; kernels with a host-metadata
 // prologue (the decode attention kernels) wait only after it.  Without the define both macros expand to nothing / a
-// plain <<<>>> launch.  Measured on a B200 (profiles/r02_step_times.json): 2-5 % off every decode step.
+// plain <<<>>> launch.
 // ------------------------------------------------------------------------------------------
 #define B200_UNPAREN(...) __VA_ARGS__
 // Per host thread: launches made while this is set carry NO programmatic-serialization attribute (b200_set_pdl).  Used for
@@ -240,6 +240,20 @@ static inline void b200_launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 blo
 #define B200_LAUNCH(kernel_in_parens, grid, block, smem, stream, ...) \
     B200_UNPAREN kernel_in_parens<<<grid, block, smem, stream>>>(__VA_ARGS__)
 #endif
+
+// SM count of the current device, for the grid heuristics of the context-less entry points (cached per device ordinal;
+// an attribute query, so it is legal while a stream is being captured)
+static inline int b200_current_sm_count() {
+    static int cached[B200_MAX_DEVICES] = {};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= B200_MAX_DEVICES) return 132;
+    if (!cached[dev]) {
+        int n = 0;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
+        cached[dev] = n;
+    }
+    return cached[dev];
+}
 
 static inline int ilog2_exact(int v) {
     int s = 0;

@@ -1,4 +1,4 @@
-// Single-token paged decode attention for sm_100a.
+// Single-token paged decode attention for sm_90a.
 //
 // Replaces the decode branch of the reference's Attention.forward (nanovllm/layers/attention.py:71-74,
 // flash_attn_with_kvcache over paged K/V).  HBM-bandwidth bound: every K/V byte of every live

@@ -372,7 +372,7 @@ bool make_chunk_map(CUtensorMap* m, const void* base, uint64_t rows) {
 template <int G>
 int launch_mma(b200_ctx* ctx, const CUtensorMap& tk, const CUtensorMap& tv, const DecodeParams& prm, long long row0, cudaStream_t st) {
     using L = MmaSmem<G>;
-    static_assert(L::kTotal <= 227 * 1024, "decode (mma) shared memory exceeds the sm_100 opt-in limit");
+    static_assert(L::kTotal <= 227 * 1024, "decode (mma) shared memory exceeds the sm_90 opt-in limit");
     auto kern = paged_decode_mma_kernel<G>;
     static B200SmemOptIn optin;
     B200_CUDA_CHECK(ctx, optin.ensure(kern, L::kTotal));

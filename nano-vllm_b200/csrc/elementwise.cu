@@ -1,4 +1,4 @@
-// The small bandwidth-bound ops around the attention operator, hand-written for sm_100a.
+// The small bandwidth-bound ops around the attention operator, hand-written for sm_90a.
 // They replace the reference's Triton KV scatter and its five @torch.compile sites (SURVEY.md 2b,
 // K1 and K5-K8): fp32 math, one rounding at every stored output (what Inductor generates on a
 // GPU), 128-bit coalesced global accesses, warp-shuffle reductions.
@@ -425,7 +425,8 @@ extern "C" int b200_silu_mul(const void* x, void* out, int rows, int inter, void
     if (rows == 0) return B200_OK;
     const int64_t total = (int64_t)rows * (inter / 8);
     int64_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    const int64_t cap = (int64_t)b200_current_sm_count() * 16;         // grid-stride beyond 16 CTAs per SM
+    if (blocks > cap) blocks = cap;
     B200_LAUNCH((silu_mul_kernel), (unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream), 
         static_cast<const __nv_bfloat16*>(x), static_cast<__nv_bfloat16*>(out), total, inter / 8);
     return b200_launch_status(nullptr);

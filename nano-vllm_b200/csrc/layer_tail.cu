@@ -1,4 +1,4 @@
-// The tail of a decoder layer in a decode step as ONE persistent kernel (tcgen05 + TMA, grid-wide barriers between phases):
+// The tail of a decoder layer in a decode step as ONE persistent kernel (wgmma + TMA, grid-wide barriers between phases):
 //
 //     o_proj  ->  residual add + RMSNorm  ->  gate_up_proj + SiluAndMul  ->  down_proj  ->  residual add + RMSNorm
 //                                                                                       [ ->  next layer's qkv_proj ]
@@ -7,34 +7,34 @@
 // (reference models/qwen3.py:87, layers/linear.py:131-156), RMSNorm.add_rms_forward (layers/layernorm.py:28-40),
 // MergedColumnParallelLinear gate_up_proj + SiluAndMul (models/qwen3.py:91-117, layers/activation.py:8-11), down_proj, the
 // next layer's input_layernorm and its QKVParallelLinear (models/qwen3.py:146-159, 72-76).  Why: in a captured decode step
-// every one of those kernels costs ~4-5 us whatever it computes (launch + fill + drain; measured, profiles/r02_*), while the
-// weights they read would stream from HBM in ~5 us for all of them together.  A grid-wide barrier inside a resident kernel
-// costs ~1 us, and the TMA producers keep running across it.
+// every one of those kernels costs a launch, a fill and a drain whatever it computes, while the weights they read would
+// stream from HBM in a few microseconds for all of them together.  A grid-wide barrier inside a resident kernel is cheaper
+// than a launch, and the TMA producer keeps running across it.
 //
-// Structure: grid = one CTA per SM (all co-resident: cooperative launch), 192 threads:
-//   warps 0-3  epilogue / normalisation (thread t owns accumulator row t = TMEM lane t)
+// Structure: grid = one CTA per SM (all co-resident: cooperative launch), 160 threads:
+//   warps 0-3  one warpgroup: wgmma m64n64k16 on both 64-row halves of an item (fp32 accumulator [128][64] in registers),
+//              frees ring slots once the MMAs that read them have retired, then epilogue / normalisation
 //   warp 4     TMA producer: a ring of 8 x {x tile [128 rows][64 k], W tile [64 n][64 k]} (128-byte swizzle)
-//   warp 5     tcgen05.mma issuer (UMMA M128 N64 K16, fp32 accumulator [128][64] in TMEM), frees ring slots with commits
 // GEMM phases walk "items" = (row block, 64-column block, k split); split-K partial sums go to an fp32 workspace and are
 // added IN SPLIT ORDER by the normalisation phase that follows (deterministic; the projection is rounded to bf16 exactly
 // where the reference's F.linear output is bf16).  Phase outputs written with ordinary stores are read by later phases
 // through TMA: writers issue fence.proxy.async + __threadfence before arriving at the grid barrier.
+#include <type_traits>
+
 #include "tc_common.cuh"
 
 namespace {
 
 using namespace b200tc;
 
-constexpr int LT_THREADS = 192;
+constexpr int LT_THREADS = 160;
 constexpr int LT_BM = 128, LT_BN = 64, LT_BK = 64;
 constexpr uint32_t LT_XT = LT_BM * 128;            // 16 KB
 constexpr uint32_t LT_WT = LT_BN * 128;            // 8 KB
 constexpr uint32_t LT_STAGE = LT_XT + LT_WT;       // 24 KB
 constexpr int LT_STAGES = 8;
 constexpr uint32_t LT_OFF_BAR = LT_STAGES * LT_STAGE;
-constexpr uint32_t LT_SMEM = LT_OFF_BAR + 256;     // full[8], empty[8], acc_full, acc_empty, tmem slot
-constexpr uint32_t LT_TMEM_COLS = 64;
-constexpr uint32_t LT_IDESC = make_idesc(LT_BM, LT_BN, false);
+constexpr uint32_t LT_SMEM = LT_OFF_BAR + 256;     // full[8], empty[8], entry generation
 
 enum { LT_EPI_PARTIAL = 0, LT_EPI_SILU = 1, LT_EPI_BF16 = 2 };
 
@@ -70,9 +70,6 @@ __device__ __forceinline__ void tma_load_2d_hint(uint32_t dst, const CUtensorMap
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;" ::
             "r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "l"(policy)
         : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ unsigned int ld_acquire_gpu(const unsigned int* p) {
     unsigned int v;
@@ -167,8 +164,6 @@ layer_tail_kernel(const __grid_constant__ CUtensorMap tm_x0, const __grid_consta
     const uint32_t base = smem_u32(smem_raw);
     if (base & 1023u) __trap();
     const uint32_t bars = base + LT_OFF_BAR;                   // full[i] = bars + 8 i, empty[i] = bars + 64 + 8 i
-    const uint32_t bar_acc_full = bars + 128, bar_acc_empty = bars + 136;
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem_raw + LT_OFF_BAR + 144);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     volatile uint32_t* gen_slot = reinterpret_cast<volatile uint32_t*>(smem_raw + LT_OFF_BAR + 152);
@@ -178,19 +173,11 @@ layer_tail_kernel(const __grid_constant__ CUtensorMap tm_x0, const __grid_consta
         // CTA's first arrival, so no barrier of this launch can have completed) and shared through smem: a thread that
         // read it on its own, later, could already see barrier 0 completed and would wait for one barrier too many
         *gen_slot = ld_acquire_gpu(p.bar_gen);
-        for (int i = 0; i < 2 * LT_STAGES; ++i) mbar_init(bars + i * 8, 1);
-        mbar_init(bar_acc_full, 1);
-        mbar_init(bar_acc_empty, 4);                           // one arrival per epilogue warp
+        for (int i = 0; i < LT_STAGES; ++i) mbar_init(bars + i * 8, 1);
+        for (int i = LT_STAGES; i < 2 * LT_STAGES; ++i) mbar_init(bars + i * 8, 4);     // one arrival per MMA warp
         mbar_fence_init();
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(bars + 144), "r"(LT_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
     const unsigned int gen0 = *gen_slot;
 
     const CUtensorMap* const mx[4] = {&tm_x0, &tm_x1, &tm_x2, &tm_x3};
@@ -227,82 +214,77 @@ layer_tail_kernel(const __grid_constant__ CUtensorMap tm_x0, const __grid_consta
                 }
             }
         }
-    } else if (warp == 5) {
-        // ---- MMA issuer ------------------------------------------------------------------------------------------------
-        if (lane == 0) {
-            uint32_t cc = 0, it = 0;                            // k tiles consumed, items issued
-            for (int ph = 0; ph < 4; ++ph) {
-                const LtGemm& g = p.g[ph];
-                if (g.n_blocks == 0) continue;
-                const int items = g.row_blocks * g.n_blocks * g.splits;
-                for (int item = blockIdx.x; item < items; item += gridDim.x, ++it) {
-                    mbar_wait(bar_acc_empty, (it & 1) ^ 1);     // the epilogue has drained the previous item's accumulator
-                    tc_fence_after();
-                    for (int kt = 0; kt < g.k_tiles; ++kt, ++cc) {
-                        const int slot = cc % LT_STAGES;
-                        mbar_wait(bars + slot * 8, (cc / LT_STAGES) & 1);
-                        tc_fence_after();
-                        const uint32_t xs = base + slot * LT_STAGE, ws = xs + LT_XT;
-#pragma unroll
-                        for (int ks = 0; ks < LT_BK / 16; ++ks)
-                            tc_mma(tmem, make_desc(xs + ks * 32, 16, 1024), make_desc(ws + ks * 32, 16, 1024), LT_IDESC, (kt > 0 || ks > 0) ? 1u : 0u);
-                        tc_commit(bars + 64 + slot * 8);
-                    }
-                    tc_commit(bar_acc_full);
-                }
-            }
-        }
     } else {
-        // ---- epilogue + normalisation warps (0-3) ----------------------------------------------------------------------
-        uint32_t it = 0;
+        // ---- MMA + epilogue + normalisation warpgroup (warps 0-3) --------------------------------------------------------
+        // acc[h][4c + 2r + e] = D[64 h + 16 warp + g + 8 r][8 c + 2 qd + e]
+        const int g8 = lane >> 2, qd = lane & 3;
+        uint32_t cc = 0;                                        // k tiles consumed (all phases)
         int next_barrier = 0;
         for (int ph = 0; ph < 4; ++ph) {
             const LtGemm& g = p.g[ph];
             if (g.n_blocks == 0) continue;
             const int items = g.row_blocks * g.n_blocks * g.splits;
-            for (int item = blockIdx.x; item < items; item += gridDim.x, ++it) {
+            for (int item = blockIdx.x; item < items; item += gridDim.x) {
                 int rb, nb, s;
                 item_coords(g, item, rb, nb, s);
-                mbar_wait(bar_acc_full, it & 1);
-                tc_fence_after();
-                float acc[LT_BN];
-                {
-                    float t0[32], t1[32];
-                    const uint32_t ta = tmem + ((uint32_t)(warp * 32) << 16);
-                    tmem_ld32(ta, t0);
-                    tmem_ld32(ta + 32, t1);
+                const bool two_halves = p.rows - rb * LT_BM > 64;
+                float acc[2][LT_BN / 2];
 #pragma unroll
-                    for (int c = 0; c < 32; ++c) { acc[c] = t0[c]; acc[32 + c] = t1[c]; }
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar_acc_empty);      // TMEM may be overwritten by the next item's first MMA
-                const int row = rb * LT_BM + tid;
-                if (row < p.rows) {
-                    if (g.epi == LT_EPI_PARTIAL) {
-                        float* dst = static_cast<float*>(g.out) + ((int64_t)s * p.rows + row) * g.out_stride + nb * LT_BN;
+                for (int h = 0; h < 2; ++h)
 #pragma unroll
-                        for (int c = 0; c < LT_BN; c += 4) *reinterpret_cast<float4*>(dst + c) = make_float4(acc[c], acc[c + 1], acc[c + 2], acc[c + 3]);
-                    } else if (g.epi == LT_EPI_SILU) {
-                        __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(g.out) + (int64_t)row * g.out_stride + nb * 32;
+                    for (int c = 0; c < LT_BN / 2; ++c) acc[h][c] = 0.f;
+                // the row-half decision is taken once, outside the MMA loop, so that every wgmma sequence is straight-line code
+                auto consume = [&](auto two) {
+                    constexpr bool TWO = decltype(two)::value;
+                    for (int kt = 0; kt < g.k_tiles; ++kt, ++cc) {
+                        const int slot = cc % LT_STAGES;
+                        mbar_wait(bars + slot * 8, (cc / LT_STAGES) & 1);
+                        const uint32_t xs = base + slot * LT_STAGE, ws = xs + LT_XT;
+                        wg_fence();
 #pragma unroll
-                        for (int c = 0; c < 32; c += 8) {
-                            float y[8];
-#pragma unroll
-                            for (int e = 0; e < 8; ++e) {
-                                const float gt = round_bf16(acc[c + e]), up = round_bf16(acc[32 + c + e]);
-                                y[e] = __fmul_rn(gt / (1.0f + expf(-gt)), up);
-                            }
-                            *reinterpret_cast<uint4*>(dst + c) = pack8(y);
+                        for (int ks = 0; ks < LT_BK / 16; ++ks) {
+                            const uint64_t bdesc = make_desc(ws + ks * 32, 16, 1024);
+                            wgmma_ss<LT_BN>(acc[0], make_desc(xs + ks * 32, 16, 1024), bdesc, 1u);
+                            if constexpr (TWO) wgmma_ss<LT_BN>(acc[1], make_desc(xs + 64 * 128 + ks * 32, 16, 1024), bdesc, 1u);
                         }
-                    } else {
-                        __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(g.out) + (int64_t)row * g.out_stride + nb * LT_BN;
+                        wg_commit();
+                        wg_wait<0>();
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(bars + 64 + slot * 8);
+                    }
+                };
+                if (two_halves) consume(std::true_type{});
+                else consume(std::false_type{});
+                acc_fence(acc[0]);
+                acc_fence(acc[1]);
 #pragma unroll
-                        for (int c = 0; c < LT_BN; c += 8) {
-                            float y[8];
+                for (int h = 0; h < 2; ++h) {
 #pragma unroll
-                            for (int e = 0; e < 8; ++e) y[e] = acc[c + e];
-                            *reinterpret_cast<uint4*>(dst + c) = pack8(y);
+                    for (int r = 0; r < 2; ++r) {
+                        const int row = rb * LT_BM + 64 * h + 16 * warp + g8 + 8 * r;
+                        if (row >= p.rows) continue;
+                        if (g.epi == LT_EPI_PARTIAL) {
+                            float* dst = static_cast<float*>(g.out) + ((int64_t)s * p.rows + row) * g.out_stride + nb * LT_BN + 2 * qd;
+#pragma unroll
+                            for (int c = 0; c < LT_BN / 8; ++c)
+                                *reinterpret_cast<float2*>(dst + 8 * c) = make_float2(acc[h][4 * c + 2 * r], acc[h][4 * c + 2 * r + 1]);
+                        } else if (g.epi == LT_EPI_SILU) {
+                            __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(g.out) + (int64_t)row * g.out_stride + nb * 32 + 2 * qd;
+#pragma unroll
+                            for (int c = 0; c < 4; ++c) {
+                                float y[2];
+#pragma unroll
+                                for (int e = 0; e < 2; ++e) {
+                                    const float gt = round_bf16(acc[h][4 * c + 2 * r + e]), up = round_bf16(acc[h][4 * (c + 4) + 2 * r + e]);
+                                    y[e] = __fmul_rn(gt / (1.0f + expf(-gt)), up);
+                                }
+                                *reinterpret_cast<uint32_t*>(dst + 8 * c) = pack_bf16x2(y[0], y[1]);
+                            }
+                        } else {
+                            __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(g.out) + (int64_t)row * g.out_stride + nb * LT_BN + 2 * qd;
+#pragma unroll
+                            for (int c = 0; c < LT_BN / 8; ++c)
+                                *reinterpret_cast<uint32_t*>(dst + 8 * c) = pack_bf16x2(acc[h][4 * c + 2 * r], acc[h][4 * c + 2 * r + 1]);
                         }
                     }
                 }
@@ -330,9 +312,6 @@ layer_tail_kernel(const __grid_constant__ CUtensorMap tm_x0, const __grid_consta
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(LT_TMEM_COLS) : "memory");
 }
 
 }  // namespace

@@ -1,12 +1,12 @@
-// Small-batch linear layers y = x W^T on the 5th-generation tensor cores, with the op that follows fused in.
+// Small-batch linear layers y = x W^T on Hopper's tensor cores (wgmma), with the op that follows fused in.
 //
-// STATUS: validated on a B200 in round 2 (tests/test_gpu_linear.py, profiles/r02_linear_microbench.json).  On the product
-// path for o_proj / down_proj of decode batches <= 128 rows (split-K) and for all four projections of the two-stream decode
-// step (models/qwen3.py::_forward_dual), where a shallow ring lets these CTAs share an SM with the attention kernel.
+// On the product path for o_proj / down_proj of decode batches <= 128 rows (split-K) and for all four projections of the
+// two-stream decode step (models/qwen3.py::_forward_dual), where a shallow ring lets these CTAs share an SM with the
+// attention kernel.
 //
 // Why: in a decode step the four projections of a layer (reference layers/linear.py:51,73,153 -> F.linear -> cuBLAS)
-// take 5-7 us each whatever the batch is (profiles/README.md), 4-8x above the time their weights need to stream from
-// HBM, and the elementwise kernels between them sit at the ~4 us floor of a tiny launch.  The levers are
+// cost several microseconds each whatever the batch is, well above the time their weights need to stream from HBM, and
+// the elementwise kernels between them sit at the floor of a tiny launch.  The levers are
 //   * weights do not depend on the previous kernel: each CTA starts streaming its W tiles before
 //     griddepcontrol.wait (programmatic dependent launch), so the HBM-bound part runs under the predecessor;
 //   * SiluAndMul (layers/activation.py:8-11) becomes the epilogue of the gate_up projection: a CTA owns BN/2 gate
@@ -15,12 +15,13 @@
 //     fp32 partials are summed IN ORDER (deterministic) by the add+RMSNorm that follows anyway
 //     (b200_add_rmsnorm_partials), which rounds the sum to bf16 exactly where the reference's GEMM output is bf16.
 //
-// Kernel: one CTA = 128 rows of x (UMMA M = 128; rows beyond `rows` are zero-filled by TMA and never stored) x BN
-// output columns x a contiguous range of 64-wide k tiles.  Warp 0 / lane 0 feeds a STAGES-deep ring of
-// {x tile [128][64], W tile [BN][64]} by TMA (128-byte swizzle, W with an L2 evict_first policy: read once per step);
-// warp 1 / lane 0 issues tcgen05.mma (both operands K-major, fp32 accumulator [128][BN] in TMEM) and releases ring
-// slots with tcgen05.commit; all four warps then read their accumulator rows with tcgen05.ld and run the epilogue.
+// Kernel: one CTA = 128 rows of x (two wgmma m64 halves; rows beyond `rows` are zero-filled by TMA and never stored, and
+// the second half is skipped when the CTA has <= 64 rows) x BN output columns x a contiguous range of 64-wide k tiles.
+// Warp 4 / lane 0 feeds a STAGES-deep ring of {x tile [128][64], W tile [BN][64]} by TMA (128-byte swizzle, W with an
+// L2 evict_first policy: read once per step); warps 0-3 (one warpgroup) issue wgmma (both operands K-major, fp32
+// accumulator in registers), release ring slots once the MMAs that read them have retired, and run the epilogue.
 #include <mutex>
+#include <type_traits>
 #include <unordered_map>
 
 #include "sample_common.cuh"
@@ -30,10 +31,11 @@ namespace {
 
 using namespace b200tc;
 
-constexpr int LM = 128;                   // rows of x per CTA (UMMA M)
+constexpr int LM = 128;                   // rows of x per CTA (two wgmma m64 halves)
 constexpr int LK = 64;                    // k extent of a ring slot: one 128-byte swizzle atom of bf16
-constexpr int L_THREADS = 128;
+constexpr int L_THREADS = 160;            // warpgroup 0 = MMA + epilogue, warp 4 = TMA producer
 constexpr uint32_t X_TILE = LM * 128;     // 16 KB
+constexpr uint32_t X_HALF = 64 * 128;     // 8 KB: rows [64, 128) of the x tile
 
 enum { EPI_BF16 = 0, EPI_SILU = 1, EPI_PARTIAL = 2, EPI_SAMPLE = 3 };
 
@@ -44,10 +46,9 @@ struct Cfg {
     static constexpr uint32_t W_TILE = BN * 128;
     static constexpr uint32_t STAGE = X_TILE + W_TILE;
     static constexpr int STAGES = !DEEP ? (BN <= 64 ? 4 : 3) : (BN <= 32 ? 8 : (BN <= 64 ? 6 : 4));
-    static constexpr uint32_t SMEM = STAGES * STAGE + 256;   // ring, then full[S], empty[S], done, TMEM slot
+    static constexpr uint32_t SMEM = STAGES * STAGE + 256;   // ring, then full[S], empty[S]
     // The ring depth actually used by a launch is LinParams::stages <= STAGES (b200_linear flags bits 4-7): the dynamic
     // shared memory of that launch is stages * STAGE + 256, so a shallow launch fits beside another kernel's CTA.
-    static constexpr uint32_t TMEM_COLS = BN < 32 ? 32 : BN;
 };
 
 struct LinParams {
@@ -74,18 +75,12 @@ __device__ __forceinline__ void tma_load_2d_hint(uint32_t dst, const CUtensorMap
 }
 // x tile shared by the CL CTAs of a cluster (neighbouring column blocks, same rows of x): each CTA fetches 128 / CL rows
 // and multicasts them into the same ring slot of every CTA of the cluster; each copy signals the mbarrier at the same
-// offset in its destination CTA.  Cuts the L2 -> SM traffic of x, the bound of these kernels at batch >= 128, by CL.
+// offset in its destination CTA.  Cuts the L2 -> SM traffic of x by CL.
 __device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, uint16_t cta_mask) {
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;" ::
             "r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
         : "memory");
-}
-// tcgen05.commit that arrives on the barrier at this offset in every CTA of the mask (a ring slot is free again only
-// when all CTAs that receive multicast data in it have consumed it)
-__device__ __forceinline__ void tc_commit_mc(uint32_t bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(cta_mask)
-                 : "memory");
 }
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
@@ -96,32 +91,15 @@ __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// this thread's accumulator row: acc[c] = D[row][c], c in [0, BN)
-template <int BN>
-__device__ __forceinline__ void load_acc_row(uint32_t taddr, float (&acc)[BN]) {
-    if constexpr (BN == 16) {
-        tmem_ld16(taddr, acc);
+// ring slot `slot` is free again in this CTA's view: one arrival per consumer warp of every CTA that received multicast
+// data in it (the producer of each CTA waits for all of them before it overwrites the slot everywhere)
+template <int CL>
+__device__ __forceinline__ void release_slot(uint32_t empty_bar, int lane) {
+    __syncwarp();
+    if constexpr (CL == 1) {
+        if (lane == 0) mbar_arrive(empty_bar);
     } else {
-#pragma unroll
-        for (int c = 0; c < BN / 32; ++c) {
-            float t[32];
-            tmem_ld32(taddr + c * 32, t);
-#pragma unroll
-            for (int e = 0; e < 32; ++e) acc[c * 32 + e] = t[e];
-        }
+        if (lane < CL) mbar_arrive_cluster(empty_bar, (uint32_t)lane);
     }
 }
 
@@ -132,15 +110,12 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
     constexpr uint16_t CL_MASK = (uint16_t)((1u << CL) - 1);
     constexpr int X_ROWS = LM / CL;                            // rows of x this CTA fetches (and multicasts when CL > 1)
     const int S = p.stages;
-    constexpr uint32_t IDESC = make_idesc(LM, BN, false);
     constexpr int BOUT = EPI == EPI_SILU ? BN / 2 : BN;       // output columns of this CTA
     extern __shared__ __align__(1024) uint8_t smem_raw[];     // 128-byte swizzle atoms need 1024-byte alignment
     const uint32_t base = smem_u32(smem_raw);
     if (base & 1023u) __trap();
     const uint32_t off_bar = (uint32_t)S * C::STAGE;
-    const uint32_t bars = base + off_bar;
-    const uint32_t bar_done = bars + 16 * S;
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem_raw + off_bar + 16 * S + 8);
+    const uint32_t bars = base + off_bar;                      // full[i] = bars + 8 i, empty[i] = bars + 8 (S + i)
 
     // let the next kernel of the stream start its own prologue (and weight prefetch) now; it still waits for this
     // grid to finish before it touches anything this grid writes (its own griddepcontrol.wait)
@@ -152,124 +127,145 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
     const int m0 = blockIdx.y * LM;
     const int kt0 = blockIdx.z * p.k_tiles;
     const int nk = p.k_tiles;
+    const bool two_halves = p.rows - m0 > 64;                 // rows [64, 128) of this CTA exist
 
     const uint32_t crank = CL > 1 ? cluster_ctarank() : 0;
     if (tid == 0) {
         for (int i = 0; i < S; ++i) mbar_init(bars + i * 8, 1);                  // full: this CTA's own expect_tx arrival
-        for (int i = S; i < 2 * S; ++i) mbar_init(bars + i * 8, CL);            // empty: one commit per CTA of the cluster
-        mbar_init(bar_done, 1);
+        for (int i = S; i < 2 * S; ++i) mbar_init(bars + i * 8, 4 * CL);        // empty: every consumer warp of the cluster
         mbar_fence_init();
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(bars + 16 * S + 8), "r"(C::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     if constexpr (CL > 1) cluster_sync_all();      // peers' barriers exist before anything is multicast at them
     else __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
-    if (warp == 0 && lane == 0) {
+    float acc[2][BN / 2];
+    if (warp == 4) {
         // ---- TMA producer --------------------------------------------------------------------------------
-        const uint64_t pol = l2_policy_evict_first();
-        auto load_w = [&](int slot, int kt) {
-            const uint32_t dst = base + slot * C::STAGE + X_TILE;
-            if constexpr (EPI == EPI_SILU) {
-                tma_load_2d_hint(dst, &tm_w, bars + slot * 8, kt * LK, blockIdx.x * BOUT, pol);
-                tma_load_2d_hint(dst + BOUT * 128, &tm_w, bars + slot * 8, kt * LK, p.up_row0 + blockIdx.x * BOUT, pol);
-            } else {
-                tma_load_2d_hint(dst, &tm_w, bars + slot * 8, kt * LK, blockIdx.x * BN, pol);
+        if (lane == 0) {
+            const uint64_t pol = l2_policy_evict_first();
+            auto load_w = [&](int slot, int kt) {
+                const uint32_t dst = base + slot * C::STAGE + X_TILE;
+                if constexpr (EPI == EPI_SILU) {
+                    tma_load_2d_hint(dst, &tm_w, bars + slot * 8, kt * LK, blockIdx.x * BOUT, pol);
+                    tma_load_2d_hint(dst + BOUT * 128, &tm_w, bars + slot * 8, kt * LK, p.up_row0 + blockIdx.x * BOUT, pol);
+                } else {
+                    tma_load_2d_hint(dst, &tm_w, bars + slot * 8, kt * LK, blockIdx.x * BN, pol);
+                }
+            };
+            auto load_x = [&](int slot, int kt) {
+                if constexpr (CL > 1)
+                    tma_load_2d_mc(base + slot * C::STAGE + crank * (X_ROWS * 128), &tm_x, bars + slot * 8, kt * LK, m0 + (int)crank * X_ROWS, CL_MASK);
+                else
+                    tma_load_2d(base + slot * C::STAGE, &tm_x, bars + slot * 8, kt * LK, m0);
+            };
+            const int pre = nk < S ? nk : S;
+            for (int i = 0; i < pre; ++i) {                      // weights first: they do not depend on the predecessor
+                mbar_expect_tx(bars + i * 8, C::STAGE);
+                load_w(i, kt0 + i);
             }
-        };
-        auto load_x = [&](int slot, int kt) {
-            if constexpr (CL > 1)
-                tma_load_2d_mc(base + slot * C::STAGE + crank * (X_ROWS * 128), &tm_x, bars + slot * 8, kt * LK, m0 + (int)crank * X_ROWS, CL_MASK);
-            else
-                tma_load_2d(base + slot * C::STAGE, &tm_x, bars + slot * 8, kt * LK, m0);
-        };
-        const int pre = nk < S ? nk : S;
-        for (int i = 0; i < pre; ++i) {                      // weights first: they do not depend on the predecessor
-            mbar_expect_tx(bars + i * 8, C::STAGE);
-            load_w(i, kt0 + i);
+            asm volatile("griddepcontrol.wait;" ::: "memory");   // x is the previous kernel's output
+            for (int i = 0; i < pre; ++i) load_x(i, kt0 + i);
+            for (int i = pre; i < nk; ++i) {
+                const int slot = i % S, round = i / S;
+                mbar_wait(bars + (S + slot) * 8, (round - 1) & 1);            // the MMAs that read this slot have retired
+                mbar_expect_tx(bars + slot * 8, C::STAGE);
+                load_w(slot, kt0 + i);
+                load_x(slot, kt0 + i);
+            }
         }
-        asm volatile("griddepcontrol.wait;" ::: "memory");   // x is the previous kernel's output
-        for (int i = 0; i < pre; ++i) load_x(i, kt0 + i);
-        for (int i = pre; i < nk; ++i) {
-            const int slot = i % S, round = i / S;
-            mbar_wait(bars + (S + slot) * 8, (round - 1) & 1);            // the MMAs that read this slot have retired
-            mbar_expect_tx(bars + slot * 8, C::STAGE);
-            load_w(slot, kt0 + i);
-            load_x(slot, kt0 + i);
-        }
-    } else if (warp == 1 && lane == 0) {
-        // ---- MMA issuer ----------------------------------------------------------------------------------
-        for (int i = 0; i < nk; ++i) {
-            const int slot = i % S, round = i / S;
-            mbar_wait(bars + slot * 8, round & 1);
-            tc_fence_after();
-            const uint32_t xs = base + slot * C::STAGE, ws = xs + X_TILE;
+    } else {
+        // ---- MMA warpgroup: one k tile in flight while the previous one retires ------------------------------------
 #pragma unroll
-            for (int ks = 0; ks < LK / 16; ++ks)
-                tc_mma(tmem, make_desc(xs + ks * 32, 16, 1024), make_desc(ws + ks * 32, 16, 1024), IDESC, (i > 0 || ks > 0) ? 1u : 0u);
-            if constexpr (CL > 1) tc_commit_mc(bars + (S + slot) * 8, CL_MASK);
-            else tc_commit(bars + (S + slot) * 8);
-        }
-        tc_commit(bar_done);
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int c = 0; c < BN / 2; ++c) acc[h][c] = 0.f;
+        // the row-half decision is taken once, outside the MMA loop, so that every wgmma sequence is straight-line code
+        auto consume = [&](auto two) {
+            constexpr bool TWO = decltype(two)::value;
+            for (int i = 0; i < nk; ++i) {
+                const int slot = i % S, round = i / S;
+                mbar_wait(bars + slot * 8, round & 1);
+                const uint32_t xs = base + slot * C::STAGE, ws = xs + X_TILE;
+                wg_fence();
+#pragma unroll
+                for (int ks = 0; ks < LK / 16; ++ks) {
+                    const uint64_t bdesc = make_desc(ws + ks * 32, 16, 1024);
+                    wgmma_ss<BN>(acc[0], make_desc(xs + ks * 32, 16, 1024), bdesc, 1u);
+                    if constexpr (TWO) wgmma_ss<BN>(acc[1], make_desc(xs + X_HALF + ks * 32, 16, 1024), bdesc, 1u);
+                }
+                wg_commit();
+                wg_wait<1>();                                  // k tile i - 1 has been read: its slot is free
+                if (i > 0) release_slot<CL>(bars + (S + (i - 1) % S) * 8, lane);
+            }
+            wg_wait<0>();
+        };
+        if (two_halves) consume(std::true_type{});
+        else consume(std::false_type{});
+        acc_fence(acc[0]);
+        acc_fence(acc[1]);
+        if (nk > 0) release_slot<CL>(bars + (S + (nk - 1) % S) * 8, lane);
     }
-    __syncwarp();
 
-    // ---- epilogue: thread t owns accumulator row t (TMEM lane t) ---------------------------------------------
-    mbar_wait(bar_done, 0);
-    tc_fence_after();
-    float acc[BN];
-    load_acc_row<BN>(tmem + ((uint32_t)(warp * 32) << 16), acc);
-    const int row = m0 + tid;
-    if constexpr (EPI == EPI_SAMPLE) {
-        // LM head + Sampler.forward in one pass (layers/embed_head.py:56-66, layers/sampler.py:7-12): this thread holds
-        // BN logits of its row; they are rounded to bf16 (the reference's logits are the bf16 output of F.linear), scored
-        // (greedy: the logit; otherwise the exponential race) and only the best (score, token) key leaves the SM.
-        if (row < p.rows) {
-            const uint64_t step = p.step + (p.step_dev ? (uint64_t)*p.step_dev : 0ull);
-            const b200sample::RowSampler rs(p.temperatures ? p.temperatures[row] : 0.f, p.seed, step, row);
-            b200sample::Best best{-INFINITY, 0x7fffffff};
-            const int n0 = blockIdx.x * BN;
+    // ---- epilogue (warpgroup 0): acc[h][4c + 2r + e] = D[64 h + 16 warp + g + 8 r][8 c + 2 qd + e] ---------------------
+    if (warp < 4) {
+        const int g = lane >> 2, qd = lane & 3;
 #pragma unroll
-            for (int c = 0; c < BN; ++c) {
-                const int col = n0 + c;
-                if (col < p.n_valid) b200sample::take(best, rs.score(round_bf16(acc[c]), p.index_offset + col), col);
-            }
-            if (best.i != 0x7fffffff)
-                atomicMax(p.keys + row, b200sample::pack_key(best.v, (uint32_t)(p.index_offset + best.i)));
-        }
-    } else if (row < p.rows) {
-        if constexpr (EPI == EPI_PARTIAL) {
-            float* dst = static_cast<float*>(p.out) + ((int64_t)blockIdx.z * p.rows + row) * p.out_stride + blockIdx.x * BN;
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
-            for (int c = 0; c < BN; c += 4) *reinterpret_cast<float4*>(dst + c) = make_float4(acc[c], acc[c + 1], acc[c + 2], acc[c + 3]);
-        } else {
-            __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(p.out) + (int64_t)row * p.out_stride + blockIdx.x * BOUT;
+            for (int r = 0; r < 2; ++r) {
+                const int row = m0 + 64 * h + 16 * warp + g + 8 * r;
+                if constexpr (EPI == EPI_SAMPLE) {
+                    // LM head + Sampler.forward in one pass (layers/embed_head.py:56-66, layers/sampler.py:7-12): this thread
+                    // holds BN/4 logits of its row; they are rounded to bf16 (the reference's logits are the bf16 output of
+                    // F.linear), scored (greedy: the logit; otherwise the exponential race) and only the best (score, token)
+                    // key of the quad's BN columns leaves the SM.
+                    unsigned long long key = 0ull;
+                    if (row < p.rows) {
+                        const uint64_t step = p.step + (p.step_dev ? (uint64_t)*p.step_dev : 0ull);
+                        const b200sample::RowSampler rs(p.temperatures ? p.temperatures[row] : 0.f, p.seed, step, row);
+                        b200sample::Best best{-INFINITY, 0x7fffffff};
+                        const int n0 = blockIdx.x * BN + 2 * qd;
 #pragma unroll
-            for (int c = 0; c < BOUT; c += 8) {
-                float y[8];
+                        for (int c = 0; c < BN / 8; ++c)
 #pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                    if constexpr (EPI == EPI_SILU) {
-                        // the reference rounds the projection to bf16 before SiluAndMul sees it (F.linear output)
-                        const float g = round_bf16(acc[c + e]), u = round_bf16(acc[BOUT + c + e]);
-                        y[e] = __fmul_rn(g / (1.0f + expf(-g)), u);
+                            for (int e = 0; e < 2; ++e) {
+                                const int col = n0 + 8 * c + e;
+                                if (col < p.n_valid) b200sample::take(best, rs.score(round_bf16(acc[h][4 * c + 2 * r + e]), p.index_offset + col), col);
+                            }
+                        if (best.i != 0x7fffffff) key = b200sample::pack_key(best.v, (uint32_t)(p.index_offset + best.i));
+                    }
+                    key = max(key, __shfl_xor_sync(0xffffffffu, key, 1));
+                    key = max(key, __shfl_xor_sync(0xffffffffu, key, 2));
+                    if (qd == 0 && key != 0ull) atomicMax(p.keys + row, key);
+                } else if (row < p.rows) {
+                    if constexpr (EPI == EPI_PARTIAL) {
+                        float* dst = static_cast<float*>(p.out) + ((int64_t)blockIdx.z * p.rows + row) * p.out_stride + blockIdx.x * BN + 2 * qd;
+#pragma unroll
+                        for (int c = 0; c < BN / 8; ++c) *reinterpret_cast<float2*>(dst + 8 * c) = make_float2(acc[h][4 * c + 2 * r], acc[h][4 * c + 2 * r + 1]);
                     } else {
-                        y[e] = acc[c + e];
+                        __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(p.out) + (int64_t)row * p.out_stride + blockIdx.x * BOUT + 2 * qd;
+#pragma unroll
+                        for (int c = 0; c < BOUT / 8; ++c) {
+                            float y[2];
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                if constexpr (EPI == EPI_SILU) {
+                                    // the reference rounds the projection to bf16 before SiluAndMul sees it (F.linear output)
+                                    const float gt = round_bf16(acc[h][4 * c + 2 * r + e]), up = round_bf16(acc[h][4 * (c + BOUT / 8) + 2 * r + e]);
+                                    y[e] = __fmul_rn(gt / (1.0f + expf(-gt)), up);
+                                } else {
+                                    y[e] = acc[h][4 * c + 2 * r + e];
+                                }
+                            }
+                            *reinterpret_cast<uint32_t*>(dst + 8 * c) = pack_bf16x2(y[0], y[1]);
+                        }
                     }
                 }
-                *reinterpret_cast<uint4*>(dst + c) = pack8(y);
             }
         }
     }
-    tc_fence_before();
+    __syncwarp();                                  // the producer warp's lanes reconverge before the .aligned cluster barrier
     if constexpr (CL > 1) cluster_sync_all();      // nobody leaves while a peer may still signal its barriers
-    else __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(C::TMEM_COLS) : "memory");
 }
 
 // RMSNorm.add_rms_forward (layers/layernorm.py:28-40) on a split-K projection: x = bf16(sum over splits, in order).

@@ -1,6 +1,6 @@
 // C-ABI entry of the prefill branch of the reference's Attention.forward (nanovllm/layers/attention.py:64-70,
-// flash_attn_varlen_func with an optional block_table).  The kernel itself is the tcgen05 / TMEM / TMA
-// flash-attention in prefill_tc.cu; this file validates arguments and forwards.
+// flash_attn_varlen_func with an optional block_table).  The kernels themselves are the wgmma / TMA
+// flash-attentions in prefill_tc.cu (default) and prefill_ws.cu; this file validates arguments and forwards.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -17,8 +17,9 @@ int b200_prefill_ws_launch(b200_ctx* ctx, int layer, const void* q, int64_t q_st
                            int num_seqs, int max_seqlen_q, int num_q_heads, int num_kv_heads, float scale,
                            cudaStream_t stream);
 
-// B200_PREFILL=ws selects the warp-specialised kernel (prefill_ws.cu: two q-heads of a GQA group per CTA, softmax
-// warpgroups / TMA warp / MMA warp), B200_PREFILL=tc the first-generation kernel (prefill_tc.cu).  Read once.
+// B200_PREFILL=ws selects the warp-specialised kernel (prefill_ws.cu: two q-heads of a GQA group per CTA, one consumer
+// warpgroup per head and a TMA producer warp), B200_PREFILL=tc (or unset) the first-generation kernel (prefill_tc.cu).
+// Read once.
 static bool use_ws_kernel() {
     static const bool ws = [] {
         const char* e = getenv("B200_PREFILL");

@@ -1,21 +1,19 @@
-// Causal varlen prefill attention on Blackwell's 5th-generation tensor cores (tcgen05 + TMEM + TMA).
+// Causal varlen prefill attention on Hopper's tensor cores (wgmma + TMA + mbarrier).
 //
 // Replaces the prefill branch of the reference's Attention.forward (nanovllm/layers/attention.py:64-70,
 // flash_attn_varlen_func with an optional block_table): packed or paged K/V, bottom-right aligned
 // causal mask (query i sees keys j <= i + len_k - len_q).
 //
-// One CTA = 128 queries of one head (UMMA M = 128, cta_group::1), key blocks of 64, two CTAs per SM:
-//   * Q, K and V tiles are staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) into shared memory;
-//     a paged K/V tile is fetched page by page through the block table with the same tensor map;
-//   * S = Q K^T : tcgen05.mma  M128 N64 K16 x 8, both operands K-major, fp32 accumulator in TMEM
-//     (two S buffers, so the next block's QK^T runs under this block's softmax);
-//   * softmax: one thread per query row reads its row with tcgen05.ld (32x32b), so row max / row sum need no
-//     shuffles; P is rounded to bf16 (as the reference's kernel does) and written to shared memory in the
-//     K-major 128B-swizzled layout the MMA expects;
-//   * O += P V : tcgen05.mma M128 N128 K16 x 4, V consumed as an MN-major operand straight from its
-//     [key][d] tile, accumulator stays in TMEM across key blocks; the running reference max only moves
-//     (and O is only rescaled through tcgen05.ld/st) when a row's max grows by more than 2^8;
-//   * completion of MMAs is tracked with tcgen05.commit -> mbarrier; one elected thread issues TMA and MMA.
+// One CTA = 128 queries of one head, two warpgroups of 64 query rows each, key blocks of 64, two CTAs per SM:
+//   * Q, K and V tiles are staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) into shared memory, K and V
+//     double-buffered so that the next block's tiles arrive under this block's math; a paged K/V tile is fetched
+//     page by page through the block table with the same tensor map;
+//   * S = Q K^T : wgmma m64n64k16 x 8 per warpgroup, both operands K-major from shared memory, fp32 in registers;
+//   * softmax in registers: a query row is held by the four threads of a quad (row max / row sum: two shuffles);
+//     P is rounded to bf16 (as the reference's kernel does) and fed to the next MMA straight from registers (the
+//     accumulator layout of S is the A-fragment layout of P);
+//   * O += P V : wgmma m64n128k16 x 4, V consumed as an MN-major operand straight from its [key][d] tile; the running
+//     reference max only moves (and O is only rescaled) when a row's max grows by more than 2^8.
 #include "tc_common.cuh"
 
 namespace {
@@ -25,19 +23,16 @@ using namespace b200tc;
 constexpr int BM = 128;
 constexpr int BN = 64;
 constexpr int D = B200_HEAD_DIM;
-constexpr int TC_THREADS = 128;
+constexpr int TC_THREADS = 256;                   // two warpgroups
 constexpr uint32_t Q_BYTES = BM * D * 2;          // 32 KB: two [128][64] halves
 constexpr uint32_t KV_BYTES = BN * D * 2;         // 16 KB: two [64][64] halves
 constexpr uint32_t Q_HALF = BM * 128;             // 16 KB
 constexpr uint32_t KV_HALF = BN * 128;            // 8 KB
-constexpr uint32_t P_BYTES = BM * BN * 2;         // 16 KB: [128][64]
 constexpr uint32_t OFF_Q = 0;
 constexpr uint32_t OFF_K = OFF_Q + Q_BYTES;       // 2 buffers
 constexpr uint32_t OFF_V = OFF_K + 2 * KV_BYTES;  // 2 buffers
-constexpr uint32_t OFF_P = OFF_V + 2 * KV_BYTES;
-constexpr uint32_t OFF_BAR = OFF_P + P_BYTES;     // 8 mbarriers + tmem slot
-constexpr uint32_t TC_SMEM = OFF_BAR + 128;       // 112.1 KB: two CTAs per SM
-constexpr uint32_t TMEM_COLS = 256;               // S0 [0,64) S1 [64,128) O [128,256)
+constexpr uint32_t OFF_BAR = OFF_V + 2 * KV_BYTES;
+constexpr uint32_t TC_SMEM = OFF_BAR + 64;        // 96.1 KB: two CTAs per SM
 constexpr float RESCALE_THRESHOLD = 8.0f;         // log2 units
 
 struct TcParams {
@@ -53,9 +48,6 @@ struct TcParams {
     float scale_log2;
 };
 
-constexpr uint32_t IDESC_QK = make_idesc(BM, BN, false);
-constexpr uint32_t IDESC_PV = make_idesc(BM, D, true);
-
 __global__ void __launch_bounds__(TC_THREADS, 2)
 prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                   const __grid_constant__ CUtensorMap tm_v, const TcParams p) {
@@ -64,10 +56,9 @@ prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
     const uint32_t base = smem_u32(smem_raw);
     if (base & 1023u) __trap();
     uint8_t* base_ptr = smem_raw;
-    const uint32_t sQ = base + OFF_Q, sK = base + OFF_K, sV = base + OFF_V, sP = base + OFF_P;
+    const uint32_t sQ = base + OFF_Q, sK = base + OFF_K, sV = base + OFF_V;
     const uint32_t bars = base + OFF_BAR;
-    const uint32_t bar_q = bars, bar_k0 = bars + 8, bar_v0 = bars + 24, bar_s0 = bars + 40, bar_o = bars + 56;
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(base_ptr + OFF_BAR + 64);
+    const uint32_t bar_q = bars, bar_k0 = bars + 8, bar_v0 = bars + 24;
 
     const int seq = blockIdx.z;
     const int head = blockIdx.y;
@@ -84,22 +75,16 @@ prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
     const int nblocks = (j_end + BN - 1) / BN;
 
     const int tid = threadIdx.x;
-    const int warp = tid >> 5;
+    const int warp = tid >> 5, lane = tid & 31;
+    const int wg = warp >> 2;                       // warpgroup: query rows [64 wg, 64 wg + 64) of the tile
+    const int g = lane >> 2, qd = lane & 3;
     const bool paged = p.block_tables != nullptr;
 
     if (tid == 0) {
-        for (int i = 0; i < 8; ++i) mbar_init(bars + i * 8, 1);
+        for (int i = 0; i < 5; ++i) mbar_init(bars + i * 8, 1);
         mbar_fence_init();
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(bars + 64), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t tmem_o = tmem + 128;
 
     auto load_kv = [&](const CUtensorMap* map, uint32_t dst, uint32_t bar, int jb) {   // one 64-key tile, both halves
         mbar_expect_tx(bar, KV_BYTES);
@@ -118,16 +103,6 @@ prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
             }
         }
     };
-    auto issue_qk = [&](int jb) {            // S[jb & 1] = Q K(jb)^T
-        const uint32_t kb = sK + (jb & 1) * KV_BYTES;
-#pragma unroll
-        for (int ks = 0; ks < D / 16; ++ks) {
-            const uint32_t hoff_q = (ks >> 2) * Q_HALF + (ks & 3) * 32;
-            const uint32_t hoff_k = (ks >> 2) * KV_HALF + (ks & 3) * 32;
-            tc_mma(tmem + (jb & 1) * BN, make_desc(sQ + hoff_q, 16, 1024), make_desc(kb + hoff_k, 16, 1024), IDESC_QK, ks > 0);
-        }
-        tc_commit(bar_s0 + (jb & 1) * 8);
-    };
 
     if (tid == 0) {
         mbar_expect_tx(bar_q, Q_BYTES);
@@ -139,135 +114,132 @@ prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
             load_kv(&tm_k, sK + KV_BYTES, bar_k0 + 8, 1);
             load_kv(&tm_v, sV + KV_BYTES, bar_v0 + 8, 1);
         }
-        mbar_wait(bar_q, 0);
-        mbar_wait(bar_k0, 0);
-        tc_fence_after();
-        issue_qk(0);
     }
 
-    const int row = mb * BM + tid;                        // in-sequence query index of this thread's row
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-    float m_ref = -INFINITY, l_sum = 0.f;
+    // this thread's two query rows (in-sequence indices) and the first row of its warp
+    const int row_lo = mb * BM + wg * 64 + (warp & 3) * 16 + g;
+    const int rows_w0 = mb * BM + wg * 64 + (warp & 3) * 16;
+    float m_ref[2] = {-INFINITY, -INFINITY}, l_sum[2] = {0.f, 0.f};
+    float o[D / 2];
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+    const uint32_t q_wg = sQ + wg * 64 * 128;
 
+    mbar_wait(bar_q, 0);
     for (int j = 0; j < nblocks; ++j) {
         const int b = j & 1;
-        if (tid == 0 && j + 1 < nblocks) {                // next block's QK^T runs under this block's softmax
-            mbar_wait(bar_k0 + ((j + 1) & 1) * 8, ((j + 1) >> 1) & 1);
-            tc_fence_after();
-            issue_qk(j + 1);
-        }
-        mbar_wait(bar_s0 + b * 8, (j >> 1) & 1);          // S(j) is in TMEM, K buffer b is free again
-        tc_fence_after();
-        if (tid == 0 && j + 2 < nblocks) load_kv(&tm_k, sK + b * KV_BYTES, bar_k0 + b * 8, j + 2);
+        const uint32_t par = (j >> 1) & 1;
 
-        // ---- this thread's row of S -------------------------------------------------------------
-        float s[BN];
-        {
-            float t0[32], t1[32];
-            tmem_ld32(tmem + lane_base + b * BN, t0);
-            tmem_ld32(tmem + lane_base + b * BN + 32, t1);
+        // ---- S = Q K(j)^T for this warpgroup's 64 rows ------------------------------------------------
+        mbar_wait(bar_k0 + b * 8, par);
+        float s[BN / 2];
+        const uint32_t kb = sK + b * KV_BYTES;
+        wg_fence();
 #pragma unroll
-            for (int c = 0; c < 32; ++c) { s[c] = t0[c] * p.scale_log2; s[32 + c] = t1[c] * p.scale_log2; }
-        }
-        const bool need_mask = (j * BN + BN > len_k) || (j * BN + BN - 1 > mb * BM + warp * 32 + off);
+        for (int ks = 0; ks < D / 16; ++ks)
+            wgmma_ss<BN>(s, make_desc(q_wg + (ks >> 2) * Q_HALF + (ks & 3) * 32, 16, 1024),
+                         make_desc(kb + (ks >> 2) * KV_HALF + (ks & 3) * 32, 16, 1024), ks > 0 ? 1u : 0u);
+        wg_commit();
+        wg_wait<0>();
+        acc_fence(s);
+
+        // s[4c + 2h + e]: row row_lo + 8h, key j*BN + 8c + 2qd + e
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) s[i] *= p.scale_log2;
+        const bool need_mask = (j * BN + BN > len_k) || (j * BN + BN - 1 > rows_w0 + off);
         if (need_mask) {
 #pragma unroll
-            for (int c = 0; c < BN; ++c) {
-                const int jj = j * BN + c;
-                if (jj >= len_k || jj > row + off) s[c] = -INFINITY;
+            for (int i = 0; i < BN / 2; ++i) {
+                const int jj = j * BN + 8 * (i >> 2) + 2 * qd + (i & 1);
+                const int r = row_lo + 8 * ((i >> 1) & 1);
+                if (jj >= len_k || jj > r + off) s[i] = -INFINITY;
             }
         }
-        float m_new = s[0];
+        float m_new[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-        for (int c = 1; c < BN; ++c) m_new = fmaxf(m_new, s[c]);
-
-        // ---- P V of the previous block must be finished before P is overwritten or O is rescaled ---------
-        if (j > 0) {
-            mbar_wait(bar_o, (j - 1) & 1);
-            tc_fence_after();
-            if (tid == 0 && j + 1 < nblocks) load_kv(&tm_v, sV + ((j + 1) & 1) * KV_BYTES, bar_v0 + ((j + 1) & 1) * 8, j + 1);
+        for (int i = 0; i < BN / 2; ++i) m_new[(i >> 1) & 1] = fmaxf(m_new[(i >> 1) & 1], s[i]);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            m_new[h] = fmaxf(m_new[h], __shfl_xor_sync(0xffffffffu, m_new[h], 1));
+            m_new[h] = fmaxf(m_new[h], __shfl_xor_sync(0xffffffffu, m_new[h], 2));
         }
+
         if (j == 0) {
-            m_ref = (m_new == -INFINITY) ? 0.f : m_new;
-        } else if (__any_sync(0xffffffffu, m_new > m_ref + RESCALE_THRESHOLD)) {
-            const float m_upd = fmaxf(m_ref, m_new);
-            const float f = fast_exp2(m_ref - m_upd);
-            m_ref = m_upd;
-            l_sum *= f;
 #pragma unroll
-            for (int q4 = 0; q4 < 4; ++q4) {
-                float o[32];
-                tmem_ld32(tmem_o + lane_base + q4 * 32, o);
+            for (int h = 0; h < 2; ++h) m_ref[h] = (m_new[h] == -INFINITY) ? 0.f : m_new[h];
+        } else if (__any_sync(0xffffffffu, m_new[0] > m_ref[0] + RESCALE_THRESHOLD || m_new[1] > m_ref[1] + RESCALE_THRESHOLD)) {
+            float f[2];
 #pragma unroll
-                for (int c = 0; c < 32; ++c) o[c] *= f;
-                tmem_st32(tmem_o + lane_base + q4 * 32, o);
+            for (int h = 0; h < 2; ++h) {
+                const float m_upd = fmaxf(m_ref[h], m_new[h]);
+                f[h] = fast_exp2(m_ref[h] - m_upd);
+                m_ref[h] = m_upd;
+                l_sum[h] *= f[h];
+            }
+#pragma unroll
+            for (int i = 0; i < D / 2; ++i) o[i] *= f[(i >> 1) & 1];
+        }
+
+        // ---- P = exp2(S - m_ref) -> bf16 A fragments (k step kk = keys 16 kk .. 16 kk + 15) -------------------
+        uint32_t pa[BN / 16][4];
+#pragma unroll
+        for (int kk = 0; kk < BN / 16; ++kk) {
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int i = 8 * kk + 2 * r;            // r: (row lo, k lo) (row hi, k lo) (row lo, k hi) (row hi, k hi)
+                const int h = r & 1;
+                const float p0 = fast_exp2(s[i] - m_ref[h]), p1 = fast_exp2(s[i + 1] - m_ref[h]);
+                l_sum[h] += p0 + p1;
+                pa[kk][r] = pack_bf16x2(p0, p1);
             }
         }
 
-        // ---- P = exp2(S - m_ref) -> bf16 -> shared memory (K-major, 128-byte swizzle) -----------------------
-        uint8_t* prow = base_ptr + OFF_P + tid * 128;
-#pragma unroll
-        for (int c8 = 0; c8 < 8; ++c8) {
-            float pv[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                pv[e] = fast_exp2(s[c8 * 8 + e] - m_ref);
-                l_sum += pv[e];
-            }
-            *reinterpret_cast<uint4*>(prow + ((c8 ^ (tid & 7)) << 4)) = pack8(pv);
-        }
+        mbar_wait(bar_v0 + b * 8, par);
         if (j * BN + BN > len_k) {
             // Tail block: V rows at keys >= len_k are not this sequence's (stale page rows, the next sequence of a packed
             // batch, anything -- possibly NaN/Inf).  Their P is exactly 0, but 0 * NaN would poison the accumulator, so
             // zero those rows of the staged tile.  A whole 128-byte row is zeroed, which is swizzle-agnostic.
-            mbar_wait(bar_v0 + b * 8, (j >> 1) & 1);
             const int first = len_k - j * BN;                               // 1..63
             uint8_t* vtile = base_ptr + OFF_V + b * KV_BYTES;
             for (int i = tid; i < (BN - first) * 16; i += TC_THREADS) {     // 16 chunks of 16 B per row: 2 halves x 8
                 const int r = first + (i >> 4), c = i & 15;
                 *reinterpret_cast<uint4*>(vtile + (c >> 3) * KV_HALF + r * 128 + ((c & 7) << 4)) = make_uint4(0, 0, 0, 0);
             }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> visible to the MMA
+            __syncthreads();
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> visible to the MMA
-        tc_fence_before();
-        __syncthreads();
 
-        // ---- O (+)= P V(j) ---------------------------------------------------------------------------
-        if (tid == 0) {
-            mbar_wait(bar_v0 + b * 8, (j >> 1) & 1);
-            tc_fence_after();
-            const uint32_t vb = sV + b * KV_BYTES;
+        // ---- O += P V(j) ---------------------------------------------------------------------------------
+        const uint32_t vb = sV + b * KV_BYTES;
+        wg_fence();
 #pragma unroll
-            for (int ks = 0; ks < BN / 16; ++ks)
-                tc_mma(tmem_o, make_desc(sP + ks * 32, 16, 1024), make_desc(vb + ks * 2048, KV_HALF, 1024), IDESC_PV,
-                       (j > 0 || ks > 0) ? 1u : 0u);
-            tc_commit(bar_o);
+        for (int kk = 0; kk < BN / 16; ++kk) wgmma_rs_bmn<D>(o, pa[kk], make_desc(vb + kk * 2048, KV_HALF, 1024), 1u);
+        wg_commit();
+        wg_wait<0>();
+        acc_fence(o);
+
+        __syncthreads();                                  // both warpgroups are done with K / V buffer b
+        if (tid == 0 && j + 2 < nblocks) {
+            load_kv(&tm_k, sK + b * KV_BYTES, bar_k0 + b * 8, j + 2);
+            load_kv(&tm_v, sV + b * KV_BYTES, bar_v0 + b * 8, j + 2);
         }
     }
 
     // ---- epilogue: O / l -> bf16 -> global ------------------------------------------------------------
-    mbar_wait(bar_o, (nblocks - 1) & 1);
-    tc_fence_after();
-    const float inv = l_sum > 0.f ? 1.f / l_sum : 0.f;
-    const bool valid = row < len_q;
-    __nv_bfloat16* dst = p.out + (int64_t)(q0 + (valid ? row : 0)) * p.out_stride + head * D;
 #pragma unroll
-    for (int q4 = 0; q4 < 4; ++q4) {
-        float o[32];
-        tmem_ld32(tmem_o + lane_base + q4 * 32, o);
-        if (valid) {
+    for (int h = 0; h < 2; ++h) {
+        float l = l_sum[h];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const float inv = l > 0.f ? 1.f / l : 0.f;
+        const int row = row_lo + 8 * h;
+        if (row < len_q) {
+            __nv_bfloat16* dst = p.out + (int64_t)(q0 + row) * p.out_stride + head * D + 2 * qd;
 #pragma unroll
-            for (int c8 = 0; c8 < 4; ++c8) {
-                float r[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) r[e] = o[c8 * 8 + e] * inv;
-                *reinterpret_cast<uint4*>(dst + q4 * 32 + c8 * 8) = pack8(r);
-            }
+            for (int c = 0; c < D / 8; ++c)
+                *reinterpret_cast<uint32_t*>(dst + 8 * c) = pack_bf16x2(o[4 * c + 2 * h] * inv, o[4 * c + 2 * h + 1] * inv);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS) : "memory");
 }
 
 }  // namespace

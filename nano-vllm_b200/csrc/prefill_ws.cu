@@ -1,24 +1,21 @@
-// Warp-specialised causal varlen prefill attention (tcgen05 + TMEM + TMA), second generation of prefill_tc.cu.
+// Warp-specialised causal varlen prefill attention (wgmma + TMA + mbarrier), second generation of prefill_tc.cu.
 //
 // Same operator (reference nanovllm/layers/attention.py:64-70: flash_attn_varlen_func, packed or paged K/V, bottom-right
-// aligned causal mask), different machine mapping.  prefill_tc.cu's CTA does MMA issue and softmax with the same 128
-// threads, so its tensor pipe idles while the rows are exponentiated (ncu: 21.6 % tensor-active, top stalls on the S / PV
-// mbarriers).  Here one CTA owns 128 queries of the TWO q-heads of a GQA group that share a kv head (every K / V tile is
-// staged once for both), and the roles are split:
+// aligned causal mask), different machine mapping.  prefill_tc.cu's warpgroups load, multiply and exponentiate in turn and
+// each CTA stages its own K / V tiles.  Here one CTA owns 64 queries of the TWO q-heads of a GQA group that share a kv head
+// (every K / V tile is staged once for both), and the roles are split:
 //
-//   warps 0-3  ("WG0")  softmax of head 0: thread r owns query row r; reads its row of S from TMEM (tcgen05.ld 32x32b),
-//                       scales / masks / exponentiates it, writes P (bf16, K-major 128-byte swizzle) to shared memory,
-//                       keeps the running reference max and row sum, rescales O in TMEM when the max moves by > 2^8
-//   warps 4-7  ("WG1")  the same for head 1
+//   warps 0-3  ("WG0")  head 0: S = Q K^T (wgmma m64n64k16 x8, fp32 in registers), scale / mask / exponentiate in
+//                       registers, P (bf16) fed to O += P V (wgmma m64n128k16 x4, A from registers, V MN-major) straight
+//                       from registers; running reference max and row sum, O rescaled in registers when the max moves by > 2^8
+//   warps 4-7  ("WG1")  the same for head 1 (idle for the last head of an odd group)
 //   warp 8              TMA producer: Q (both heads) once, then a 3-deep ring of K and V tiles (64 keys), paged tiles
-//                       page by page through the block table
-//   warp 9              tcgen05.mma issuer: S_t = Q_t K^T (M128 N64 K16 x8) into a double-buffered S per head, O_t += P_t V
-//                       (M128 N128 K16 x4, V as an MN-major operand) -- QK^T of block j+1 is issued before the PV of block j,
-//                       so the tensor pipe works on the next scores of both heads while both warpgroups exponentiate
+//                       page by page through the block table; a slot is refilled once every consumer warp has released it
 //
-// TMEM (512 columns): S[head][buf] 4 x 64, O[head] 2 x 128.  Shared memory: Q 2 x 32 KB, K 3 x 16 KB, V 3 x 16 KB,
-// P 2 x 16 KB = 192 KB, one CTA per SM.  Arithmetic and rounding points are those of prefill_tc.cu (P rounded to bf16 as
-// the reference's kernel does, fp32 accumulation, one rounding of the output).
+// The two warpgroups run independently on the shared ring, so the tensor pipe works on one head's MMAs while the other
+// head is exponentiating.  Shared memory: Q 2 x 16 KB, K 3 x 16 KB, V 3 x 16 KB = 128 KB, one CTA per SM.  Arithmetic and
+// rounding points are those of prefill_tc.cu (P rounded to bf16 as the reference's kernel does, fp32 accumulation, one
+// rounding of the output); with POLY half of the exponentials run as a polynomial on the FMA pipe.
 #include <cstdlib>
 
 #include "tc_common.cuh"
@@ -27,33 +24,25 @@ namespace {
 
 using namespace b200tc;
 
-constexpr int BM = 128, BN = 64, D = B200_HEAD_DIM;
-constexpr int WS_THREADS = 320;                    // 2 softmax warpgroups + producer warp + MMA warp
+constexpr int BM = 64, BN = 64, D = B200_HEAD_DIM;
+constexpr int WS_THREADS = 288;                    // 2 consumer warpgroups + producer warp
 constexpr int KV_STAGES = 3;
-constexpr uint32_t Q_BYTES = BM * D * 2;           // 32 KB per head: two [128][64] halves
-constexpr uint32_t Q_HALF = BM * 128;
-constexpr uint32_t KV_BYTES = BN * D * 2;          // 16 KB: two [64][64] halves
-constexpr uint32_t KV_HALF = BN * 128;
-constexpr uint32_t P_BYTES = BM * BN * 2;          // 16 KB
+constexpr uint32_t Q_HALF = BM * 128;              // 8 KB: [64 rows][64 dims]
+constexpr uint32_t Q_BYTES = 2 * Q_HALF;           // 16 KB per head
+constexpr uint32_t KV_HALF = BN * 128;             // 8 KB
+constexpr uint32_t KV_BYTES = 2 * KV_HALF;         // 16 KB: two [64][64] halves
 constexpr uint32_t OFF_Q = 0;                                        // 2 heads
 constexpr uint32_t OFF_K = OFF_Q + 2 * Q_BYTES;
 constexpr uint32_t OFF_V = OFF_K + KV_STAGES * KV_BYTES;
-constexpr uint32_t OFF_P = OFF_V + KV_STAGES * KV_BYTES;             // 2 heads
-constexpr uint32_t OFF_BAR = OFF_P + 2 * P_BYTES;
-constexpr uint32_t WS_SMEM = OFF_BAR + 256;
-constexpr uint32_t TMEM_COLS = 512;                // S[t][b] at (t * 2 + b) * 64, O[t] at 256 + t * 128
+constexpr uint32_t OFF_BAR = OFF_V + KV_STAGES * KV_BYTES;
+constexpr uint32_t WS_SMEM = OFF_BAR + 128;
 constexpr float RESCALE_THRESHOLD = 8.0f;          // log2 units
-constexpr uint32_t IDESC_QK = make_idesc(BM, BN, false);
-constexpr uint32_t IDESC_PV = make_idesc(BM, D, true);
 
 // barrier slots (8 bytes each) from OFF_BAR
 constexpr uint32_t B_Q = 0;                        // Q tiles landed
-constexpr uint32_t B_KFULL = 1, B_KEMPTY = 4, B_VFULL = 7, B_VEMPTY = 10;   // 3 each
-constexpr uint32_t B_SFULL = 13;                   // [t][b]: 13 + t * 2 + b
-constexpr uint32_t B_PREADY = 17;                  // [t]: P_t written (and S_t read, O_t rescaled): 128 arrivals
-constexpr uint32_t B_ODONE = 19;                   // [t]: the PV MMA of the block has completed
-constexpr uint32_t B_COUNT = 21;
-constexpr uint32_t TMEM_SLOT = B_COUNT * 8;        // byte offset of the tcgen05.alloc result
+constexpr uint32_t B_KFULL = 1, B_VFULL = 4;       // 3 each
+constexpr uint32_t B_EMPTY = 7;                    // 3: one arrival per consumer warp once its PV of the slot has retired
+constexpr uint32_t B_COUNT = 10;
 
 struct WsParams {
     const int32_t* cu_q;
@@ -68,9 +57,9 @@ struct WsParams {
     float scale_log2;
 };
 
-// 2^x for x <= ~8 on the FMA/ALU pipes instead of the 16-per-clock MUFU unit (the softmax of this kernel is MUFU-bound: one
-// exp2 per score).  Cody-Waite split x = n + f, f in [0, 1), and a degree-3 minimax polynomial for 2^f (relative error
-// < 1e-4, far inside the bf16 rounding P gets anyway); the exponent is added into the float's exponent field.
+// 2^x for x <= ~8 on the FMA/ALU pipes instead of the MUFU unit (the softmax is MUFU-bound: one exp2 per score).
+// Cody-Waite split x = n + f, f in [0, 1), and a degree-3 minimax polynomial for 2^f (relative error < 1e-4, far inside the
+// bf16 rounding P gets anyway); the exponent is added into the float's exponent field.
 __device__ __forceinline__ float exp2_poly(float x) {
     const float xc = fmaxf(x, -120.0f);
     const float n = floorf(xc);
@@ -82,28 +71,23 @@ __device__ __forceinline__ float exp2_poly(float x) {
     return x < -120.0f ? 0.f : y;                      // masked scores (-inf) must give exactly 0
 }
 
-__device__ __forceinline__ void mbar_arrive_ws(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-
 template <bool POLY>
 __global__ void __launch_bounds__(WS_THREADS, 1)
 prefill_ws_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                   const __grid_constant__ CUtensorMap tm_v, const WsParams p) {
     B200_PDL_SYNC();
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    extern __shared__ __align__(1024) uint8_t smem_raw[];   // 128-byte swizzle atoms need 1024-byte alignment
     const uint32_t base = smem_u32(smem_raw);
     if (base & 1023u) __trap();
     const uint32_t bars = base + OFF_BAR;
     auto bar = [&](uint32_t i) { return bars + i * 8; };
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem_raw + OFF_BAR + TMEM_SLOT);
 
     const int seq = blockIdx.z;
     const int g_heads = p.hq / p.hkv;                      // q heads per kv head
     const int pairs_per_kv = (g_heads + 1) / 2;
     const int kvh = blockIdx.y / pairs_per_kv;
     const int head0 = kvh * g_heads + (blockIdx.y % pairs_per_kv) * 2;
-    const bool two = (head0 + 1) < (kvh + 1) * g_heads;    // an odd group leaves the second tile of its last pair idle
+    const bool two = (head0 + 1) < (kvh + 1) * g_heads;    // an odd group leaves the second warpgroup of its last pair idle
     const int mb = gridDim.x - 1 - blockIdx.x;             // longest tiles first
     const int q0 = p.cu_q[seq];
     const int len_q = p.cu_q[seq + 1] - q0;
@@ -119,17 +103,11 @@ prefill_ws_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
     const bool paged = p.block_tables != nullptr;
 
     if (tid == 0) {
-        for (uint32_t i = 0; i < B_COUNT; ++i) mbar_init(bar(i), (i == B_PREADY || i == B_PREADY + 1) ? 128 : 1);
+        for (uint32_t i = 0; i < B_EMPTY; ++i) mbar_init(bar(i), 1);
+        for (uint32_t i = B_EMPTY; i < B_COUNT; ++i) mbar_init(bar(i), two ? 8 : 4);
         mbar_fence_init();
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(bars + TMEM_SLOT), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
     if (warp == 8) {
         // ---- TMA producer -------------------------------------------------------------------------------------------
@@ -158,168 +136,137 @@ prefill_ws_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
             };
             for (int j = 0; j < nblocks; ++j) {
                 const int s = j % KV_STAGES;
-                if (j >= KV_STAGES) {
-                    const uint32_t par = ((j / KV_STAGES) - 1) & 1;
-                    mbar_wait(bar(B_KEMPTY + s), par);
-                    load_kv(&tm_k, base + OFF_K + s * KV_BYTES, bar(B_KFULL + s), j);
-                    mbar_wait(bar(B_VEMPTY + s), par);
-                    load_kv(&tm_v, base + OFF_V + s * KV_BYTES, bar(B_VFULL + s), j);
-                } else {
-                    load_kv(&tm_k, base + OFF_K + s * KV_BYTES, bar(B_KFULL + s), j);
-                    load_kv(&tm_v, base + OFF_V + s * KV_BYTES, bar(B_VFULL + s), j);
-                }
+                if (j >= KV_STAGES) mbar_wait(bar(B_EMPTY + s), ((j / KV_STAGES) - 1) & 1);
+                load_kv(&tm_k, base + OFF_K + s * KV_BYTES, bar(B_KFULL + s), j);
+                load_kv(&tm_v, base + OFF_V + s * KV_BYTES, bar(B_VFULL + s), j);
             }
         }
-    } else if (warp == 9) {
-        // ---- MMA issuer ---------------------------------------------------------------------------------------------------
-        if (lane == 0) {
-            const int nt = two ? 2 : 1;
-            auto issue_qk = [&](int j) {                   // S[t][j & 1] = Q_t K(j)^T for both heads, then K slot free
-                const int s = j % KV_STAGES;
-                mbar_wait(bar(B_KFULL + s), (j / KV_STAGES) & 1);
-                tc_fence_after();
-                const uint32_t kb = base + OFF_K + s * KV_BYTES;
-                for (int t = 0; t < nt; ++t) {
-                    const uint32_t qb = base + OFF_Q + t * Q_BYTES;
-#pragma unroll
-                    for (int ks = 0; ks < D / 16; ++ks) {
-                        const uint32_t hq_off = (ks >> 2) * Q_HALF + (ks & 3) * 32;
-                        const uint32_t hk_off = (ks >> 2) * KV_HALF + (ks & 3) * 32;
-                        tc_mma(tmem + (t * 2 + (j & 1)) * BN, make_desc(qb + hq_off, 16, 1024), make_desc(kb + hk_off, 16, 1024), IDESC_QK, ks > 0);
-                    }
-                    tc_commit(bar(B_SFULL + t * 2 + (j & 1)));
-                }
-                tc_commit(bar(B_KEMPTY + s));
-            };
-            mbar_wait(bar(B_Q), 0);
-            tc_fence_after();
-            issue_qk(0);
-            for (int j = 0; j < nblocks; ++j) {
-                if (j + 1 < nblocks) issue_qk(j + 1);      // the next scores run under this block's softmax
-                const int s = j % KV_STAGES;
-                mbar_wait(bar(B_VFULL + s), (j / KV_STAGES) & 1);
-                const uint32_t vb = base + OFF_V + s * KV_BYTES;
-                for (int t = 0; t < nt; ++t) {
-                    mbar_wait(bar(B_PREADY + t), j & 1);   // P_t(j) is in shared memory, S_t(j) has been read, O_t is rescaled
-                    tc_fence_after();
-                    const uint32_t pb = base + OFF_P + t * P_BYTES;
-#pragma unroll
-                    for (int ks = 0; ks < BN / 16; ++ks)
-                        tc_mma(tmem + 256 + t * D, make_desc(pb + ks * 32, 16, 1024), make_desc(vb + ks * 2048, KV_HALF, 1024), IDESC_PV,
-                               (j > 0 || ks > 0) ? 1u : 0u);
-                    tc_commit(bar(B_ODONE + t));
-                }
-                tc_commit(bar(B_VEMPTY + s));
-            }
-        }
-    } else {
-        // ---- softmax warpgroups ---------------------------------------------------------------------------------------------
-        const int t = warp >> 2;                           // head of the pair
-        const int r = tid & 127;                           // query row within the tile = TMEM lane
-        if (t == 0 || two) {
-            const int wq = warp & 3;
-            const uint32_t lane_base = (uint32_t)(wq * 32) << 16;
-            const uint32_t tmem_o = tmem + 256 + t * D;
-            const int row = mb * BM + r;                   // in-sequence query index
-            uint8_t* prow = smem_raw + OFF_P + t * P_BYTES + r * 128;
-            float m_ref = -INFINITY, l_sum = 0.f;
-            for (int j = 0; j < nblocks; ++j) {
-                const int b = j & 1;
-                mbar_wait(bar(B_SFULL + t * 2 + b), (j >> 1) & 1);
-                tc_fence_after();
-                float s[BN];
-                {
-                    float t0[32], t1[32];
-                    tmem_ld32(tmem + lane_base + (t * 2 + b) * BN, t0);
-                    tmem_ld32(tmem + lane_base + (t * 2 + b) * BN + 32, t1);
-#pragma unroll
-                    for (int c = 0; c < 32; ++c) { s[c] = t0[c] * p.scale_log2; s[32 + c] = t1[c] * p.scale_log2; }
-                }
-                const bool need_mask = (j * BN + BN > len_k) || (j * BN + BN - 1 > mb * BM + wq * 32 + off);
-                if (need_mask) {
-#pragma unroll
-                    for (int c = 0; c < BN; ++c) {
-                        const int jj = j * BN + c;
-                        if (jj >= len_k || jj > row + off) s[c] = -INFINITY;
-                    }
-                }
-                float m_new = s[0];
-#pragma unroll
-                for (int c = 1; c < BN; ++c) m_new = fmaxf(m_new, s[c]);
+        return;
+    }
 
-                if (j > 0) {                               // PV_t(j-1) finished: P_t may be overwritten, O_t is stable
-                    mbar_wait(bar(B_ODONE + t), (j - 1) & 1);
-                    tc_fence_after();
-                }
-                if (j == 0) {
-                    m_ref = (m_new == -INFINITY) ? 0.f : m_new;
-                } else if (__any_sync(0xffffffffu, m_new > m_ref + RESCALE_THRESHOLD)) {
-                    const float m_upd = fmaxf(m_ref, m_new);
-                    const float f = fast_exp2(m_ref - m_upd);
-                    m_ref = m_upd;
-                    l_sum *= f;
+    // ---- consumer warpgroup t: q-head head0 + t ------------------------------------------------------------------------
+    const int t = warp >> 2;
+    if (t == 1 && !two) return;
+    const int g = lane >> 2, qd = lane & 3;
+    const int row_lo = mb * BM + (warp & 3) * 16 + g;      // this thread's two query rows: row_lo, row_lo + 8
+    const int rows_w0 = mb * BM + (warp & 3) * 16;
+    const uint32_t sQ = base + OFF_Q + t * Q_BYTES;
+    float m_ref[2] = {-INFINITY, -INFINITY}, l_sum[2] = {0.f, 0.f};
+    float o[D / 2];
 #pragma unroll
-                    for (int q4 = 0; q4 < 4; ++q4) {
-                        float o[32];
-                        tmem_ld32(tmem_o + lane_base + q4 * 32, o);
+    for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+
+    mbar_wait(bar(B_Q), 0);
+    for (int j = 0; j < nblocks; ++j) {
+        const int s = j % KV_STAGES;
+        const uint32_t par = (j / KV_STAGES) & 1;
+
+        // ---- S = Q K(j)^T ---------------------------------------------------------------------------------------
+        mbar_wait(bar(B_KFULL + s), par);
+        float sc[BN / 2];
+        const uint32_t kb = base + OFF_K + s * KV_BYTES;
+        wg_fence();
 #pragma unroll
-                        for (int c = 0; c < 32; ++c) o[c] *= f;
-                        tmem_st32(tmem_o + lane_base + q4 * 32, o);
-                    }
-                }
+        for (int ks = 0; ks < D / 16; ++ks)
+            wgmma_ss<BN>(sc, make_desc(sQ + (ks >> 2) * Q_HALF + (ks & 3) * 32, 16, 1024),
+                         make_desc(kb + (ks >> 2) * KV_HALF + (ks & 3) * 32, 16, 1024), ks > 0 ? 1u : 0u);
+        wg_commit();
+        wg_wait<0>();
+        acc_fence(sc);
+
+        // sc[4c + 2h + e]: row row_lo + 8h, key j*BN + 8c + 2qd + e
 #pragma unroll
-                for (int c8 = 0; c8 < 8; ++c8) {
-                    float pv[8];
+        for (int i = 0; i < BN / 2; ++i) sc[i] *= p.scale_log2;
+        const bool need_mask = (j * BN + BN > len_k) || (j * BN + BN - 1 > rows_w0 + off);
+        if (need_mask) {
 #pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        // every other score goes through the polynomial: halves the MUFU load, the FMA pipe has room
-                        pv[e] = (POLY && (e & 1)) ? exp2_poly(s[c8 * 8 + e] - m_ref) : fast_exp2(s[c8 * 8 + e] - m_ref);
-                        l_sum += pv[e];
-                    }
-                    *reinterpret_cast<uint4*>(prow + ((c8 ^ (r & 7)) << 4)) = pack8(pv);
-                }
-                if (j * BN + BN > len_k) {
-                    // tail block: V rows at keys >= len_k are not this sequence's (stale page rows / the next packed sequence):
-                    // P is exactly 0 there but 0 * NaN would poison the accumulator -> zero those rows of the staged tile.  Both
-                    // warpgroups do it (same values) so that each one's arrival below covers the tile its own PV MMA reads.
-                    const int sv = j % KV_STAGES;
-                    mbar_wait(bar(B_VFULL + sv), (j / KV_STAGES) & 1);
-                    const int first = len_k - j * BN;                               // 1..63
-                    uint8_t* vtile = smem_raw + OFF_V + sv * KV_BYTES;
-                    for (int i = r; i < (BN - first) * 16; i += 128) {
-                        const int rr = first + (i >> 4), c = i & 15;
-                        *reinterpret_cast<uint4*>(vtile + (c >> 3) * KV_HALF + rr * 128 + ((c & 7) << 4)) = make_uint4(0, 0, 0, 0);
-                    }
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");        // P (and V) writes -> visible to the MMA
-                tc_fence_before();
-                mbar_arrive_ws(bar(B_PREADY + t));
+            for (int i = 0; i < BN / 2; ++i) {
+                const int jj = j * BN + 8 * (i >> 2) + 2 * qd + (i & 1);
+                const int r = row_lo + 8 * ((i >> 1) & 1);
+                if (jj >= len_k || jj > r + off) sc[i] = -INFINITY;
             }
-            // ---- epilogue: O / l -> bf16 -> global --------------------------------------------------------------------------
-            mbar_wait(bar(B_ODONE + t), (nblocks - 1) & 1);
-            tc_fence_after();
-            const float inv = l_sum > 0.f ? 1.f / l_sum : 0.f;
-            const bool valid = row < len_q;
-            __nv_bfloat16* dst = p.out + (int64_t)(q0 + (valid ? row : 0)) * p.out_stride + (head0 + t) * D;
+        }
+        float m_new[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-            for (int q4 = 0; q4 < 4; ++q4) {
-                float o[32];
-                tmem_ld32(tmem_o + lane_base + q4 * 32, o);
-                if (valid) {
+        for (int i = 0; i < BN / 2; ++i) m_new[(i >> 1) & 1] = fmaxf(m_new[(i >> 1) & 1], sc[i]);
 #pragma unroll
-                    for (int c8 = 0; c8 < 4; ++c8) {
-                        float rr[8];
+        for (int h = 0; h < 2; ++h) {
+            m_new[h] = fmaxf(m_new[h], __shfl_xor_sync(0xffffffffu, m_new[h], 1));
+            m_new[h] = fmaxf(m_new[h], __shfl_xor_sync(0xffffffffu, m_new[h], 2));
+        }
+        if (j == 0) {
 #pragma unroll
-                        for (int e = 0; e < 8; ++e) rr[e] = o[c8 * 8 + e] * inv;
-                        *reinterpret_cast<uint4*>(dst + q4 * 32 + c8 * 8) = pack8(rr);
-                    }
-                }
+            for (int h = 0; h < 2; ++h) m_ref[h] = (m_new[h] == -INFINITY) ? 0.f : m_new[h];
+        } else if (__any_sync(0xffffffffu, m_new[0] > m_ref[0] + RESCALE_THRESHOLD || m_new[1] > m_ref[1] + RESCALE_THRESHOLD)) {
+            float f[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const float m_upd = fmaxf(m_ref[h], m_new[h]);
+                f[h] = fast_exp2(m_ref[h] - m_upd);
+                m_ref[h] = m_upd;
+                l_sum[h] *= f[h];
             }
+#pragma unroll
+            for (int i = 0; i < D / 2; ++i) o[i] *= f[(i >> 1) & 1];
+        }
+
+        // ---- P = exp2(S - m_ref) -> bf16 A fragments (k step kk = keys 16 kk .. 16 kk + 15) -------------------
+        uint32_t pa[BN / 16][4];
+#pragma unroll
+        for (int kk = 0; kk < BN / 16; ++kk) {
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int i = 8 * kk + 2 * r;            // r: (row lo, k lo) (row hi, k lo) (row lo, k hi) (row hi, k hi)
+                const int h = r & 1;
+                const float p0 = fast_exp2(sc[i] - m_ref[h]);
+                const float p1 = POLY ? exp2_poly(sc[i + 1] - m_ref[h]) : fast_exp2(sc[i + 1] - m_ref[h]);
+                l_sum[h] += p0 + p1;
+                pa[kk][r] = pack_bf16x2(p0, p1);
+            }
+        }
+
+        mbar_wait(bar(B_VFULL + s), par);
+        if (j * BN + BN > len_k) {
+            // Tail block: V rows at keys >= len_k are not this sequence's (stale page rows, the next sequence of a packed
+            // batch, anything -- possibly NaN/Inf).  Their P is exactly 0, but 0 * NaN would poison the accumulator, so
+            // zero those rows of the staged tile (each warpgroup writes the same zeros, then orders them before its MMA).
+            const int first = len_k - j * BN;                               // 1..63
+            uint8_t* vtile = smem_raw + OFF_V + s * KV_BYTES;
+            for (int i = tid & 127; i < (BN - first) * 16; i += 128) {       // 16 chunks of 16 B per row: 2 halves x 8
+                const int r = first + (i >> 4), c = i & 15;
+                *reinterpret_cast<uint4*>(vtile + (c >> 3) * KV_HALF + r * 128 + ((c & 7) << 4)) = make_uint4(0, 0, 0, 0);
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> visible to the MMA
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + t) : "memory");        // this warpgroup only
+        }
+
+        // ---- O += P V(j) ---------------------------------------------------------------------------------------
+        const uint32_t vb = base + OFF_V + s * KV_BYTES;
+        wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < BN / 16; ++kk) wgmma_rs_bmn<D>(o, pa[kk], make_desc(vb + kk * 2048, KV_HALF, 1024), 1u);
+        wg_commit();
+        wg_wait<0>();
+        acc_fence(o);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar(B_EMPTY + s));     // this warp no longer reads slot s
+    }
+
+    // ---- epilogue: O / l -> bf16 -> global ------------------------------------------------------------
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float l = l_sum[h];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const float inv = l > 0.f ? 1.f / l : 0.f;
+        const int row = row_lo + 8 * h;
+        if (row < len_q) {
+            __nv_bfloat16* dst = p.out + (int64_t)(q0 + row) * p.out_stride + (head0 + t) * D + 2 * qd;
+#pragma unroll
+            for (int c = 0; c < D / 8; ++c)
+                *reinterpret_cast<uint32_t*>(dst + 8 * c) = pack_bf16x2(o[4 * c + 2 * h] * inv, o[4 * c + 2 * h + 1] * inv);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS) : "memory");
 }
 
 }  // namespace
@@ -360,6 +307,7 @@ int b200_prefill_ws_launch(b200_ctx* ctx, int layer, const void* q, int64_t q_st
             !make_map(&tv, v, (uint64_t)num_kv_heads * D, (uint64_t)total_k, (uint64_t)v_stride0, BN))
             return B200_EUNSUPPORTED;
     }
+    // B200_PREFILL_POLY=0 keeps every exponential on the MUFU unit (A/B of the polynomial half)
     static const bool poly = [] { const char* e = getenv("B200_PREFILL_POLY"); return e ? atoi(e) != 0 : true; }();
     static B200SmemOptIn optin_poly, optin_mufu;
     const int g_heads = num_q_heads / num_kv_heads;

@@ -1,4 +1,4 @@
-// Token sampling for sm_100a: replaces Sampler.forward (nanovllm/layers/sampler.py:7-12, an
+// Token sampling for sm_90a: replaces Sampler.forward (nanovllm/layers/sampler.py:7-12, an
 // Inductor-compiled softmax + exponential race) and adds the greedy branch (temperature == 0)
 // the north-star requires.  The logits are streamed once with 128-bit loads and only a running
 // (value, index) maximum is kept: nothing of size [rows, vocab] is materialised.
@@ -112,7 +112,7 @@ extern "C" int b200_sample(const void* logits, int logits_is_fp32, int64_t logit
     if (rows == 0) return B200_OK;
     int splits = 1;
     if (rows <= MAX_ROWS_SPLIT) {
-        splits = (148 * 8) / rows;
+        splits = (b200_current_sm_count() * 8) / rows;          // about eight CTAs per SM
         splits = splits < 1 ? 1 : (splits > MAX_SPLITS ? MAX_SPLITS : splits);
         while (splits > 1 && vocab / splits < 2048) --splits;      // keep slices worth a CTA
     }

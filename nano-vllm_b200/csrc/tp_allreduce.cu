@@ -1,4 +1,4 @@
-// Tensor-parallel exchange fused with the op that always follows it, over NVLink peer memory (sm_100a).
+// Tensor-parallel exchange fused with the op that always follows it, over NVLink peer memory (sm_90a).
 //
 // Replaces, for a decode step, the pair
 //     dist.all_reduce(y)                          RowParallelLinear.forward, reference layers/linear.py:152-156

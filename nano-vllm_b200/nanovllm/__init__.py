@@ -1,4 +1,4 @@
-"""nanovllm API (LLM / SamplingParams) on the B200-native paged-attention path.
+"""nanovllm API (LLM / SamplingParams) on the H100-native paged-attention path.
 
 Same public surface as the reference package (reference nanovllm/__init__.py:1-2), so
 ``from nanovllm import LLM, SamplingParams`` in the reference's bench.py / example.py keeps

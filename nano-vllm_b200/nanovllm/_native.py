@@ -37,7 +37,7 @@ SIGNATURES = {
     "b200_embedding": (_i, [_vp, _vp, _vp, _i, _i, _i64, _vp]),
     "b200_gather_tokens": (_i, [_vp, _vp, _vp, _i, _vp]),
     "b200_sample": (_i, [_vp, _i, _i64, _vp, _i, _i, _i64, _u64, _u64, _vp, _vp, _vp, _vp]),
-    # decode-size projections on tcgen05 (csrc/linear_tc.cu) and the fused LM head / layer tail experiments
+    # decode-size projections on wgmma (csrc/linear_tc.cu) and the fused LM head / layer tail experiments
     "b200_linear": (_i, [_vp, _i64, _vp, _vp, _i64, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "b200_add_rmsnorm_partials": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _f, _i, _vp]),
     "b200_lm_head_sample": (_i, [_vp, _i64, _vp, _i, _i, _i, _vp, _i64, _u64, _u64, _vp, _vp, _vp, _vp, _i, _i, _vp]),
@@ -112,7 +112,7 @@ def handle(device: int | None = None) -> Handle:
     if _handle is None:
         import torch
         if not torch.cuda.is_available():
-            raise B200Error("no CUDA device: the B200 path has no CPU fallback")
+            raise B200Error("no CUDA device: the GPU path has no CPU fallback")
         _handle = Handle(torch.cuda.current_device() if device is None else device)
     return _handle
 

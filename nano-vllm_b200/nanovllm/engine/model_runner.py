@@ -5,7 +5,7 @@ Same contract as the reference's ModelRunner (nanovllm/engine/model_runner.py:15
 is_prefill) -> list[int]`` returns one token id per sequence; one process per GPU, one thread,
 everything on the current stream, one device->host sync per step.
 
-B200-first differences (DESIGN.md "runner"):
+Differences from the reference (DESIGN.md "runner"):
 * per-step metadata travels in ONE pinned staging buffer (two of them, ping-pong, so step N+1 can be staged
   while step N runs) and ONE host->device copy into static device buffers (the reference builds seven pinned
   tensors and seven copies per step);
@@ -80,7 +80,7 @@ class ModelRunner:
         self.graph_kernels: dict[int, int] = {}
 
         if not torch.cuda.is_available():
-            raise nat.B200Error("ModelRunner needs a CUDA device: the B200 path has no CPU fallback")
+            raise nat.B200Error("ModelRunner needs a CUDA device: the GPU path has no CPU fallback")
         local = int(os.environ.get("LOCAL_RANK", rank))
         # Debug / CI knob: B200_TP_BACKEND=gloo with B200_TP_ONE_DEVICE=1 runs all tensor-parallel ranks on ONE GPU
         # (time-sliced processes, collectives through gloo, eager only): the sharding, the vocab-parallel sampling and

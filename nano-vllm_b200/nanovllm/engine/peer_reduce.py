@@ -36,8 +36,8 @@ class PeerReduce:
         self.handle = symm.rendezvous(self.raw, dist.group.WORLD)
         self.bases_dev = int(self.handle.buffer_ptrs_dev)
         # Sum inside the NVSwitch (multimem.ld_reduce on the multicast mapping of the same buffer) when there is a multicast
-        # mapping: every rank then pulls rows x hidden x 2 bytes per exchange instead of world x that.  Measured on B200
-        # (profiles/r02_bench_tp{2,8}_*.json): +3.7 % at 8 ranks, -2.5 % at 2 ranks, so the default (B200_TP_ALLREDUCE=auto)
+        # mapping: every rank then pulls rows x hidden x 2 bytes per exchange instead of world x that, at the price of a
+        # round trip through the switch, which only pays off with several peers, so the default (B200_TP_ALLREDUCE=auto)
         # uses it from 4 ranks up; "peer" / "nvls" force one of the two, "nccl" bypasses this module.
         self.mc_ptr = int(getattr(self.handle, "multicast_ptr", 0) or 0)
         mode = os.environ.get("B200_TP_ALLREDUCE", "auto")

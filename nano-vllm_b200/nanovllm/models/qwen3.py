@@ -1,4 +1,4 @@
-"""Qwen3 dense decoder on the B200 kernels (reference nanovllm/models/qwen3.py:14-216).
+"""Qwen3 dense decoder on the libb200attn kernels (reference nanovllm/models/qwen3.py:14-216).
 
 Same architecture and the same rounding points as the reference's GPU path: GQA with per-head q/k
 RMSNorm before NeoX RoPE, SwiGLU MLP, fused residual-add + RMSNorm; bf16 tensors between ops, fp32
@@ -70,20 +70,20 @@ class Qwen3ForCausalLM:
         self.kv_size = self.num_kv_heads * self.head_dim
         self.tie = bool(getattr(c, "tie_word_embeddings", False))
         # b200_paged_decode_fused folds q/k-norm + RoPE + KV append into the decode kernel (one launch less per
-        # layer).  Measured on the benchmark shapes it saves 1-2 us per layer up to batch ~128 and loses 2 us at
-        # batch 256 (the extra per-segment math lands on warps that are already busy), so it is used for decode
-        # batches up to this many rows; it exists for head groups <= 2 only.
+        # layer).  The extra per-segment math lands on warps that are already busy, which costs more than the saved
+        # launch at large batches, so it is used for decode batches up to this many rows; it exists for head groups
+        # <= 2 only.
         self.fused_decode_max_batch = 128 if self.num_heads // self.num_kv_heads <= 2 else 0
         if "B200_FUSED_DECODE_MAX" in os.environ and self.fused_decode_max_batch:      # tuning knob (e.g. under TP)
             self.fused_decode_max_batch = int(os.environ["B200_FUSED_DECODE_MAX"])
         self.peer = None        # engine/peer_reduce.PeerReduce when tensor parallel over NVLink peer memory
-        # Decode-size projections (measured per batch size on a B200, profiles/r02_step_times.json, r02_linear_microbench.json):
+        # Decode-size projections (profiles/step_time.py compares the policies step for step):
         #   B200_LINEAR=auto (default): the two row-parallel projections (o_proj, down_proj) of decode steps of up to 128 rows
-        #       run on tcgen05 with split-K 8 and the add+RMSNorm that follows consumes the fp32 partials in split order
-        #       (csrc/linear_tc.cu): 4-21 % off the step at batch <= 128; at batch 256 and for the wide projections
-        #       (qkv, gate_up) the library GEMM is faster, so those stay cuBLAS, as under tensor parallelism;
-        #   cublas: every projection through the library;  rows / tc: force the tcgen05 path for o/down / all four;
-        #   gu: only gate_up + SiluAndMul on tcgen05 (one launch less per layer), the rest through the library.
+        #       run on wgmma with split-K 8 and the add+RMSNorm that follows consumes the fp32 partials in split order
+        #       (csrc/linear_tc.cu), so that all SMs stream weights; the wide projections (qkv, gate_up) stay cuBLAS, as
+        #       under tensor parallelism;
+        #   cublas: every projection through the library;  rows / tc: force the wgmma path for o/down / all four;
+        #   gu: only gate_up + SiluAndMul on wgmma (one launch less per layer), the rest through the library.
         #   B200_LINEAR_CFG = "qkv_bn,gate_up_bn,o_bn,o_splits,down_bn,down_splits,pdl".
         mode = os.environ.get("B200_LINEAR", "auto")
         self.tc_linear = mode in ("tc", "rows") or (mode == "auto" and tp_size == 1)
@@ -92,21 +92,19 @@ class Qwen3ForCausalLM:
         self.tc_gate_up_max = int(os.environ.get("B200_LINEAR_GU_MAX_ROWS", "256"))
         self.tc_cfg = [int(v) for v in os.environ.get("B200_LINEAR_CFG", "64,64,64,8,64,8,1").split(",")]
         self.tc_max_rows = int(os.environ.get("B200_LINEAR_MAX_ROWS", "128" if mode == "auto" else "256"))
-        # above 128 rows a CTA row block is added, so fewer k splits cover the SMs (micro-benchmark at 256 rows, split 4 vs 8:
-        # o_proj 7.6 vs 11.2 us, down_proj 8.8 vs 12.5 us incl. the add-norm); B200_LINEAR_SPLITS_BIG overrides.  In the captured step
-        # B200_LINEAR_MAX_ROWS=256 with split 4 measured level with the library path (3 790 vs 3 774 us at 256 rows), so 128 stays.
+        # above 128 rows a CTA row block is added, so fewer k splits cover the SMs; B200_LINEAR_SPLITS_BIG overrides.
         self.tc_big_splits = int(os.environ.get("B200_LINEAR_SPLITS_BIG", "4"))
         fit = lambda k, s: next(d for d in range(max(1, min(s, k // 64)), 0, -1) if (k // 64) % d == 0)     # split-K factors must divide the k tiles
         tcc = self.tc_cfg
         if self.q_size % 64 or self.inter % 64 or self.hidden % tcc[2] or self.hidden % tcc[4]:
-            self.tc_linear = False                # shapes the tcgen05 kernel does not tile: library GEMMs
+            self.tc_linear = False                # shapes the wgmma kernel does not tile: library GEMMs
         else:
             tcc[3], tcc[5] = fit(self.q_size, tcc[3]), fit(self.inter, tcc[5])
             self.tc_big = (fit(self.q_size, min(tcc[3], self.tc_big_splits)), fit(self.inter, min(tcc[5], self.tc_big_splits)))
         # B200_TAIL=mega: in decode steps of up to 256 rows on one GPU, everything between two attention kernels
         # (o_proj, add+norm, gate_up+SiluAndMul, down_proj, add+norm, the next layer's qkv_proj) is ONE persistent launch
-        # (csrc/layer_tail.cu) instead of seven.  Measured 58-70 us per layer against 30 us for the chain (r02_layer_tail_microbench.json):
-        # kept as an opt-in experiment, off by default.
+        # (csrc/layer_tail.cu) instead of seven.  Every phase is an all-to-all dependency (a norm needs whole rows), so a grid
+        # barrier and a pipeline refill per phase compete with a launch boundary under PDL: an opt-in experiment, off by default.
         self.mega_tail = os.environ.get("B200_TAIL", "") == "mega" and tp_size == 1
         self.mega_rows = 256
         want = [int(v) for v in os.environ.get("B200_TAIL_SPLITS", "8,8").split(",")]
@@ -116,12 +114,12 @@ class Qwen3ForCausalLM:
         # Two-stream decode step (B200_DUAL, _forward_dual): a decode batch of >= dual_min rows is cut into two halves that
         # run on two streams, half a layer out of phase: while one half is in its HBM-bound attention kernel (fp32-FMA pipe +
         # bulk copies, ~155 KB of shared memory, one CTA per SM) the other half's latency-bound projection chain runs on
-        # the SAME SMs -- tcgen05 + TMA, a 3-slot ring (~72 KB) and ~10k registers, which is what the attention CTA leaves
+        # the SAME SMs -- wgmma + TMA, a 3-slot ring (~72 KB) and ~30k registers, which is what the attention CTA leaves
         # free.  Attention kernels never overlap each other (an event chain orders them), so HBM always has one streaming
         # kernel and the chain of the other half hides under it.  One GPU, head groups <= 2 (the FMA decode kernel).
         #   B200_DUAL_CFG = "qkv_bn,gate_up_bn,o_bn,o_splits,down_bn,down_splits,ring_slots"
-        # Measured (profiles/r02_two_stream.json): the co-residency works (both = 71.7 us vs 56.9 + 35.5 serial per half layer) but
-        # a half batch costs more than half, so the step is 8 % slower at 256 rows: off by default.
+        # A half batch costs more than half of a full one (attention and the projection chain are both latency bound at
+        # these sizes), so this is off by default.
         dual = os.environ.get("B200_DUAL", "0")
         self.dual = dual not in ("0", "", "off") and tp_size == 1 and self.num_heads // self.num_kv_heads <= 2
         self.dual_min = int(os.environ.get("B200_DUAL_MIN", "144"))
@@ -204,7 +202,7 @@ class Qwen3ForCausalLM:
     # ---- forward -------------------------------------------------------------------------------
     def _row_linear(self, x: torch.Tensor, w: torch.Tensor, tc=None):
         """Row-parallel GEMM (o_proj / down_proj).  Returns (partial, where): where is True when the partial sits in
-        the peer-mapped buffer, "parts" when it is the fp32 split-K partials of the tcgen05 path."""
+        the peer-mapped buffer, "parts" when it is the fp32 split-K partials of the wgmma path."""
         peer = self.peer
         if tc is not None and self.tp_size == 1:
             return ops.linear(x, w, ops.EPI_PARTIAL, tc[0], tc[1], pdl=bool(self.tc_cfg[6])), "parts"
@@ -287,9 +285,9 @@ class Qwen3ForCausalLM:
 
     def _forward_dual(self, input_ids: torch.Tensor, positions: torch.Tensor, ctx) -> torch.Tensor:
         """Decode step as two half batches on two streams, half a layer out of phase (see __init__).  Per half and layer:
-        add+norm(split-K partials) -> qkv (tcgen05) -> attention [no PDL, after the other half's attention] -> o_proj split-K
-        [no PDL] -> add+norm -> gate_up+SiluAndMul (tcgen05) -> down_proj split-K.  Same rounding points as the single-stream
-        tcgen05 path (split-K partials summed in split order by the add+norm)."""
+        add+norm(split-K partials) -> qkv (wgmma) -> attention [no PDL, after the other half's attention] -> o_proj split-K
+        [no PDL] -> add+norm -> gate_up+SiluAndMul (wgmma) -> down_proj split-K.  Same rounding points as the single-stream
+        wgmma path (split-K partials summed in split order by the add+norm)."""
         import contextlib
         n = input_ids.shape[0]
         h0 = (n + 1) // 2

@@ -1,7 +1,7 @@
 """Tensor-facing wrappers over the C ABI: pass data_ptr()s, strides and the current stream.
 
 PyTorch is plumbing here (device memory + streams); every function below is one
-launch of a hand-written sm_100a kernel in libb200attn.so.
+launch of a hand-written sm_90a kernel in libb200attn.so.
 """
 from __future__ import annotations
 
@@ -237,7 +237,7 @@ def tokens_from_keys(keys: torch.Tensor) -> torch.Tensor:
     return 0xffffffff - (keys & 0xffffffff)
 
 
-# ---- decode-size projections on tcgen05 (csrc/linear_tc.cu) -----------------------------------------------------------
+# ---- decode-size projections on wgmma (csrc/linear_tc.cu) -------------------------------------------------------------
 EPI_BF16, EPI_SILU, EPI_PARTIAL = 0, 1, 2
 
 
@@ -256,7 +256,7 @@ class pdl_off:
 def linear(x: torch.Tensor, w: torch.Tensor, epilogue: int = EPI_BF16, block_n: int = 32, k_splits: int = 1,
            pdl: bool = False, out: torch.Tensor | None = None, shallow: bool = False, cluster: int = 1,
            stages: int = 0) -> torch.Tensor:
-    """x [rows, k] @ w[n, k]^T on tcgen05.  EPI_SILU: w = [gate; up] rows, returns silu(gate) * up [rows, n/2];
+    """x [rows, k] @ w[n, k]^T on wgmma.  EPI_SILU: w = [gate; up] rows, returns silu(gate) * up [rows, n/2];
     EPI_PARTIAL: returns fp32 [k_splits, rows, n] partial sums for ``add_rmsnorm_partials``.
     ``stages`` (0 = default): ring depth in slots of 16 KB + block_n * 128 B."""
     _need(x, torch.bfloat16, "x"); _need(w, torch.bfloat16, "w")

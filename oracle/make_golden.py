@@ -1,9 +1,9 @@
-"""Generate tests/golden/* by running the REFERENCE's own code in the build container.
+"""Generate tests/golden/* by running the REFERENCE's own code.
 
-    TORCH_COMPILE_DISABLE=1 python oracle/make_golden.py            # needs /root/reference
+    TORCH_COMPILE_DISABLE=1 python oracle/make_golden.py            # needs the reference under oracle/_ref
 
-The reference is Python, so it can be imported here (never on the GPU box: nothing at test time
-reads /root/reference).  What gets pinned:
+The reference is Python and is staged under oracle/_ref (oracle/install_reference.py); nothing at test
+time reads it, the tests read what this script stored.  What gets pinned:
 
 1. hash_kat.json          BlockManager.compute_hash known answers          (block_manager.py:35-41)
 2. trace_<workload>.json  step-by-step digests of the reference Scheduler / BlockManager /
@@ -32,7 +32,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden")
-REF = os.environ.get("NANOVLLM_REFERENCE", "/root/reference")
+REF = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref")   # oracle/install_reference.py
 sys.path.insert(0, ROOT)
 
 
@@ -146,6 +146,16 @@ def step_record(seqs, is_prefill: bool, meta: dict) -> list:
     return [int(is_prefill), len(seqs), int(ntok), digest(*book), digest(*md)]
 
 
+COMPACT_CHUNK = 32
+
+
+def compact_steps(steps) -> str:
+    """A workload's step records as one string of 8-hex-digit hashes, one per chunk of COMPACT_CHUNK consecutive steps
+    (keeps the fuzz fixtures small; a differing step still changes its chunk's hash)."""
+    return "".join(hashlib.sha256(json.dumps(steps[i:i + COMPACT_CHUNK]).encode()).hexdigest()[:8]
+                   for i in range(0, len(steps), COMPACT_CHUNK))
+
+
 def drive(make_seq, scheduler, block_size, build_meta, w) -> dict:
     """Run one workload to completion; identical for the reference classes and the product's."""
     for p, (t, mt, ie) in zip(w["prompts"], w["sps"]):
@@ -234,7 +244,8 @@ def gen_traces(torch, only=None):
 
 
 def fuzz_reference(torch, seed: int, n: int, out_path: str):
-    """Reference side of the differential test: run the reference's classes over fuzz_workloads(seed, n)."""
+    """Reference side of the differential test: run the reference's classes over fuzz_workloads(seed, n); the step records
+    are stored compacted (compact_steps)."""
     import itertools
     from nanovllm.engine.scheduler import Scheduler
     from nanovllm.engine.sequence import Sequence
@@ -246,9 +257,10 @@ def fuzz_reference(torch, seed: int, n: int, out_path: str):
         Sequence.counter = itertools.count()
         make_seq = lambda p, t, mt, ie: Sequence(p, SamplingParams(temperature=t, max_tokens=mt, ignore_eos=ie))
         rec = drive(make_seq, Scheduler(cfg), cfg.kvcache_block_size, reference_meta_builder(torch, cfg.kvcache_block_size), w)
+        rec["steps"] = compact_steps(rec["steps"])
         results.append(rec)
     with open(out_path, "w") as f:
-        json.dump(results, f)
+        json.dump(results, f, separators=(",", ":"))
 
 
 def api_surface(pkg) -> dict:
@@ -372,7 +384,7 @@ def main():
         for preset in only[1:]:
             gen_model(torch, preset)
         return
-    if only and only[0] == "--fuzz":         # `make_golden.py --fuzz SEED N OUT.json` (tests/test_differential_fuzz.py)
+    if only and only[0] == "--fuzz":         # `make_golden.py --fuzz SEED 150 tests/golden/fuzz_seedSEED.json`
         fuzz_reference(torch, int(only[1]), int(only[2]), only[3])
         return
     if only:

@@ -4,7 +4,7 @@ TEST INFRASTRUCTURE / REPORTED BASELINE ONLY (see oracle/__init__.py) -- nothing
     python oracle/ref_cpu_arm.py <model_dir> <reps> <budget_seconds> [n_seqs]
 
 Runs, in a process of its own (the reference and the product both own the package name ``nanovllm``), the unmodified
-reference installed under baseline/_ref:
+reference installed under oracle/_ref:
   * its Scheduler / BlockManager / Sequence                         (engine/scheduler.py, block_manager.py, sequence.py)
   * its ModelRunner.prepare_prefill / prepare_decode, unbound       (engine/model_runner.py:123-188; pin_memory/.cuda()
     neutralised, exactly like oracle/make_golden.py does)
@@ -28,7 +28,7 @@ import time
 import types
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 def main():

@@ -1,4 +1,4 @@
-"""BASELINE.json configs[2] sanity + timing: Qwen3-8B dims (random init), block_size=16, prefix cache on, one B200.
+"""BASELINE.json configs[2] sanity + timing: Qwen3-8B dims (random init), block_size=16, prefix cache on, one GPU.
 
     NANOVLLM_ALLOW_RANDOM_INIT=1 python profiles/config3_8b.py [num_seqs] [max_tokens]
 
@@ -48,7 +48,7 @@ def main():
     # weights the logits are nearly flat, so a one-ulp difference between batch shapes can flip an argmax;
     # the agreement length is reported, not asserted
     same = [agree(outs[0]["token_ids"], outs[-2]["token_ids"]), agree(outs[1]["token_ids"], outs[-1]["token_ids"])]
-    print(json.dumps({"config": "Qwen3-8B dims random-init bf16, block_size 16, prefix cache, 1xB200", "seqs": n,
+    print(json.dumps({"config": "Qwen3-8B dims random-init bf16, block_size 16, prefix cache, 1 GPU", "seqs": n,
                       "max_tokens": max_tokens, "output_tok_s": n * max_tokens / dt, "seconds": dt, "init_s": init_s,
                       "kv_blocks": llm.config.num_kvcache_blocks, "cached_hashes": len(bm.hash_to_block_id),
                       "duplicate_prompt_agreement_tokens": same}))

@@ -1,4 +1,4 @@
-"""Does a tcgen05 projection chain hide under the decode-attention kernel of ANOTHER stream on the same SMs?
+"""Does a wgmma projection chain hide under the decode-attention kernel of ANOTHER stream on the same SMs?
 
     python profiles/dual_microbench.py [rows per half, default 128] [ring slots, default 3]
 
@@ -6,7 +6,7 @@ Times, per layer (CUDA events, graph replay of 28 layers, median of 20 replays),
 batch-256 context mix cut in two:
   attn     b200_paged_decode_fused of one half batch alone
   chain    the six non-attention kernels of one half batch alone (add+norm, qkv, o split-K, add+norm, gate_up+SiluAndMul,
-           down split-K; tcgen05 with the given ring depth)
+           down split-K; wgmma with the given ring depth)
   both     the two on two streams at once (what one phase of the two-stream decode step does)
 `both` ~ max(attn, chain) means the chain's CTAs do share the SMs with the attention CTAs; `both` ~ attn + chain means
 they do not (shared memory / registers / carve-out) and the two-stream step cannot win.

@@ -7,7 +7,7 @@ SURVEY.md 8(f) rows 1 and 4: once the GPU step is fast, what the host does per s
 the metadata builders (prepare_prefill / prepare_decode / prepare_block_tables), Scheduler.postprocess (+ hash_blocks) --
 bounds tokens/s unless it hides under the GPU step.  This replays a workload with fake tokens (oracle/make_golden.py's driver,
 the one the golden traces were made with, so both sides take identical decisions) and times the three parts per step with
-perf_counter.  "ref" = the unmodified reference from baseline/_ref (its prepare_* run unbound with pin_memory / .cuda()
+perf_counter.  "ref" = the unmodified reference from oracle/_ref (its prepare_* run unbound with pin_memory / .cuda()
 neutralised: what it does on the host before the copies); "ours" = nanovllm/engine of this repo (flat-array BlockManager,
 vectorised numpy builders writing one pinned staging buffer -- the staging copy itself is not part of this number).
 Both sides run in this process's CPU, one thread, one after the other, each in its own interpreter (they share a package name).
@@ -21,7 +21,7 @@ import time
 import types
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 def run_side(side: str, name: str) -> dict:
@@ -93,7 +93,7 @@ def main():
         row = {}
         for side in ("ours", "ref"):
             if side == "ref" and not os.path.isdir(os.path.join(REF, "nanovllm")):
-                row[side] = "baseline/_ref absent"
+                row[side] = "oracle/_ref absent"
                 continue
             env = dict(os.environ, OMP_NUM_THREADS="1")
             r = subprocess.run([sys.executable, os.path.abspath(__file__), side, name], capture_output=True, text=True, env=env)

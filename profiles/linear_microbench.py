@@ -1,10 +1,10 @@
-"""Staged tcgen05 linear (csrc/linear_tc.cu) against the library path it would replace, at Qwen3-0.6B decode shapes.
+"""Staged wgmma linear (csrc/linear_tc.cu) against the library path it would replace, at Qwen3-0.6B decode shapes.
 
-    timeout 600 python profiles/linear_microbench.py > gpurun_out/linear_microbench.json
+    python profiles/linear_microbench.py > linear_microbench.json
 
 A configuration the library refuses (unsupported shape) is recorded as null; results are flushed per batch size.
 
-Each measurement is one CUDA-graph replay of the op over 16 distinct weight sets (more bytes than the 126 MB L2 for the
+Each measurement is one CUDA-graph replay of the op over 16 distinct weight sets (more bytes than the 50 MB L2 for the
 large shapes, as in a real step where every layer has its own weights), CUDA events around the replay, best of 5.
 """
 import itertools

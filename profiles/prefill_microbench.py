@@ -1,6 +1,6 @@
 """Prefill attention kernel alone on the benchmark's prefill shapes (packed, causal, Hq16/Hkv8/D128).
 
-    B200_PREFILL=tc|hmma python profiles/prefill_microbench.py [--paged]
+    B200_PREFILL=tc|ws python profiles/prefill_microbench.py [--paged]
 
 Sequence lengths are those of the benchmark's first prefill step (31 prompts, 15 705 tokens).
 FLOPs = sum_s 4 * Hq * D * (len_q*len_k - len_q^2/2)   (SURVEY.md 8d).
@@ -63,7 +63,7 @@ def main():
         e1.record()
         torch.cuda.synchronize()
         best = min(best, e0.elapsed_time(e1))
-    print(json.dumps(dict(impl=os.environ.get("B200_PREFILL", "hmma"), paged=args.paged, seqs=len(lens), tokens=tot, us=best * 1000,
+    print(json.dumps(dict(impl=os.environ.get("B200_PREFILL", "tc"), paged=args.paged, seqs=len(lens), tokens=tot, us=best * 1000,
                           tflops=flops / (best * 1e-3) / 1e12)))
 
 

@@ -151,7 +151,7 @@ def main():
     if rank == 0:
         hf = llm.config.hf_config
         line = {
-            "config": {3: "Qwen3-8B dims random-init bf16, 512 seqs, kvcache_block_size 16, shared 600-token prefix (prefix cache on), 1xB200",
+            "config": {3: "Qwen3-8B dims random-init bf16, 512 seqs, kvcache_block_size 16, shared 600-token prefix (prefix cache on), 1 GPU",
                        4: "Qwen3-8B dims random-init bf16, tensor_parallel_size 4, 1024 seqs in/out U[100,1024], max_num_seqs 512 (mixed prefill+decode)",
                        5: "Qwen3-32B dims random-init bf16, tensor_parallel_size 8, 128 seqs, 8192-token prompts, 1024 output tokens, max_model_len 9472"}[cfg],
             "n_gpus": world, "output_tokens": sum(max_tokens), "prompt_tokens": sum(len(p) for p in prompts),

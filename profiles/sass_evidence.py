@@ -1,7 +1,7 @@
 """Static evidence from the built library (no GPU needed): per kernel, registers / shared memory and the SASS mnemonics that
-show which hardware paths it uses (tcgen05 MMA, TMEM loads/stores, TMA tensor / bulk copies, multicast, multimem, PDL).
+show which hardware paths it uses (wgmma, TMA tensor / bulk copies, multicast, multimem, PDL).
 
-    python profiles/sass_evidence.py > profiles/r02_sass_evidence.txt
+    python profiles/sass_evidence.py
 """
 import os
 import re
@@ -11,7 +11,7 @@ from collections import Counter, OrderedDict
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "nano-vllm_b200", "lib", "libb200attn.so")
-WATCH = ["UTCHMMA", "UTCBAR", "LDTM", "STTM", "UTMALDG", "UTMAPF", "UBLKCP", "SYNCS", "MULTICAST", "MULTIMEM", "LDGMC", "REDG", "ACQBULK", "PREEXIT",
+WATCH = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMAPF", "UBLKCP", "SYNCS", "MULTICAST", "MULTIMEM", "LDGMC", "REDG", "ACQBULK", "PREEXIT",
          "HMMA", "LDSM", "MUFU.EX2", "CCTL", "ERRBAR", "ATOM"]
 
 
@@ -52,7 +52,7 @@ def main():
                 if op.startswith(w) or ("." + w) in op:
                     counts[cur][w] += 1
     names = demangle(list(usage))
-    print(f"# {os.path.relpath(LIB, ROOT)}: {len(usage)} kernels (sm_100a).  Columns: registers/thread, static shared bytes, SASS instructions, watched mnemonics")
+    print(f"# {os.path.relpath(LIB, ROOT)}: {len(usage)} kernels (sm_90a).  Columns: registers/thread, static shared bytes, SASS instructions, watched mnemonics")
     rows = []
     for k, (reg, stack, sh, local) in usage.items():
         c = counts.get(k, Counter())

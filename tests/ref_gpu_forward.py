@@ -1,4 +1,4 @@
-"""Runs the UNMODIFIED reference model (baseline/_ref: its Qwen3ForCausalLM, its flash-attn Attention.forward,
+"""Runs the UNMODIFIED reference model (oracle/_ref: its Qwen3ForCausalLM, its flash-attn Attention.forward,
 its Triton store_kvcache, its loader) on cuda:0 over a teacher-forced serving script and saves the logits.
 TEST INFRASTRUCTURE ONLY -- executed as a subprocess by tests/test_gpu_reference_forward.py because the reference
 and the product both own the package name ``nanovllm``.
@@ -17,7 +17,7 @@ import os
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 def main():

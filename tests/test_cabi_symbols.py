@@ -159,7 +159,7 @@ def test_argument_validation_needs_no_gpu():
     assert lib.b200_allreduce_add_rmsnorm_nvls(p, None, 0, 0, p, p, p, 0, 2, p, p, p, 1, 1024, 1e-6, None) == EINVAL
     assert lib.b200_allreduce_add_rmsnorm_nvls(p, p, 0, 0, p, p, p, 0, 9, p, p, p, 1, 1024, 1e-6, None) == EINVAL
     assert lib.b200_allreduce_add_rmsnorm_nvls(p, p, 0, 0, p, p, p, 0, 2, p, p, p, 0, 1024, 1e-6, None) == 0
-    # tcgen05 linear layer: k a multiple of 64, split-K only with the partial-sum epilogue, block sizes from the list
+    # wgmma linear layer: k a multiple of 64, split-K only with the partial-sum epilogue, block sizes from the list
     assert lib.b200_linear(None, 64, p, p, 64, 1, 64, 64, 0, 32, 1, 0, None) == EINVAL
     assert lib.b200_linear(p, 64, p, p, 64, 1, 64, 96, 0, 32, 1, 0, None) == EUNSUPPORTED
     assert lib.b200_linear(p, 128, p, p, 64, 1, 64, 128, 0, 32, 2, 0, None) == EINVAL

@@ -1,8 +1,8 @@
-"""The numbers DESIGN.md quotes are the ones in the committed evidence files (profiles/), and those files carry every key the
-bench contract names.  No GPU: this only reads JSON / text that GPU runs left behind."""
+"""The numbers DESIGN.md quotes are the ones in the committed evidence file (profiles/h100_bench_n1.json), which records the
+GPU they were measured on and carries every key the benchmark line names.  No GPU: this only reads JSON that a GPU run left
+behind."""
 import json
 import os
-import re
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 P = lambda *a: os.path.join(ROOT, "profiles", *a)
@@ -14,13 +14,16 @@ def _fmt(n: float) -> str:
 
 
 def test_headline_bench_line_is_complete_and_consistent():
-    d = json.load(open(P("r02_bench_n1.json")))
+    rec = json.load(open(P("h100_bench_n1.json")))
+    gpu = rec["gpu"]
+    assert "H100" in gpu["name"] and float(gpu["power_limit_w"]) > 0
+    d = rec["bench"]
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline",
               "dtype", "data", "config", "e2e", "gpu_launches", "clocks", "roofline", "cpu_baseline", "parity"):
         assert k in d, k
     assert d["n_gpus"] == 1 and d["warmup"] >= 3 and d["higher_is_better"] is True and "workload" in d["config"]
     r = d["roofline"]
-    assert r["bound"] == "hbm" and abs(r["frac"] - r["achieved"] / r["peak"]) < 1e-9 and r["traffic"] > 0
+    assert r["bound"] == "hbm" and abs(r["frac"] - r["achieved"] / r["peak"]) < 1e-9
     assert d["e2e"]["h2d_bytes_per_step"] > 0 and d["e2e"]["d2h_bytes_per_step"] > 0 and d["e2e"]["value"] < d["value"]
     assert d["gpu_launches"] > 0 and d["parity"]["ok"] is True
     assert d["cpu_baseline"]["kind"] in ("reference", "port") and d["cpu_baseline"]["cores"] >= 1
@@ -28,25 +31,4 @@ def test_headline_bench_line_is_complete_and_consistent():
     design = open(os.path.join(ROOT, "DESIGN.md")).read()
     assert _fmt(d["value"]) in design and _fmt(d["e2e"]["value"]) in design, "DESIGN.md section 6 quotes another run"
     assert f"{r['frac']:.3f}" in design
-
-
-def test_ncu_summary_is_the_source_of_the_traffic_figure():
-    text = open(P("r02_decode_kernel_ncu.txt")).read()
-    rd = float(re.search(r"dram__bytes_read\.sum\s+([0-9.]+)\s+Mbyte", text).group(1))
-    wr = float(re.search(r"dram__bytes_write\.sum\s+([0-9.]+)\s+Mbyte", text).group(1))
-    d = json.load(open(P("r02_bench_n1.json")))
-    assert abs(d["roofline"]["traffic"] - (rd + wr) * 1e6) < 1e3
-    assert 0.99 < (rd + wr) / 587.2 < 1.02, "DRAM traffic of the batch-256 launch should equal its algorithmic bytes"
-
-
-def test_scaling_and_config_lines_carry_parity():
-    for f, n in (("r02_bench_tp2b.json", 2), ("r02_bench_tp4_nvls.json", 4)):
-        d = json.load(open(P(f)))
-        assert d["n_gpus"] == n and d["parity"]["ok"] and d["parity"]["ranks_agree"] and d["parity"]["ranks"] == n
-    d8 = json.load(open(P("r02_bench_tp8b.json")))["lines"]["default"]
-    assert d8["n_gpus"] == 8 and d8["parity"]["ok"] and d8["parity"]["tp_exchange"] == "nvls"
-    for cfg, gpus in ((3, 1), (4, 4), (5, 8)):
-        c = json.load(open(P(f"r02_config{cfg}.json")))
-        assert c["n_gpus"] == gpus and c["output_tok_s"] > 0 and c["decode_kernel"]["bound"] == "hbm"
-        if gpus > 1:
-            assert c["parity"]["ranks_agree"] is True
+    assert gpu["name"] in design and f"{float(gpu['power_limit_w']):.0f} W" in design, "DESIGN.md names another GPU"

@@ -151,7 +151,7 @@ def test_paged_decode_wide_groups_ignore_stale_rows(ops, hq, hkv, bs, lens):
 @pytest.mark.parametrize("bs", [16, 64, 256])
 def test_prefill_paged_ignores_stale_rows(ops, bs):
     """Paged prefill (prefill_tc.cu) stages whole 64-key tiles; keys >= len_k of the last tile are stale page rows (or
-    page 0 when the tile runs past the block table).  NaN there must not reach the tcgen05 accumulator."""
+    page 0 when the tile runs past the block table).  NaN there must not reach the tensor-core accumulator."""
     hq, hkv = 8, 2
     len_k = [300, 77, 130, 40, 65]
     len_q = [44, 77, 1, 13, 65]
@@ -322,7 +322,7 @@ def test_prefill_paged_prefix_and_chunk(ops, bs):
 
 def test_prefill_long_causal_and_rescale(ops):
     """Many key blocks per query tile, and scores whose running maximum keeps growing by far more than 2^8, so the
-    in-TMEM accumulator is rescaled repeatedly (the lazy-rescale path of the tcgen05 kernel)."""
+    register accumulator is rescaled repeatedly (the lazy-rescale path of the wgmma kernel)."""
     hq, hkv = 4, 2
     lens = [1500, 900, 257]
     tot = sum(lens)

@@ -1,9 +1,9 @@
-"""Parity tests for the tcgen05 linear layer (csrc/linear_tc.cu): the decode-size projections of the product path (o_proj /
+"""Parity tests for the wgmma linear layer (csrc/linear_tc.cu): the decode-size projections of the product path (o_proj /
 down_proj split-K for batches <= 128 rows; all four in the two-stream decode step) and the fused LM-head + sampling kernel.
 
 Reference for every case: torch fp32 matmul of the same bf16 inputs, rounded where the reference rounds
 (F.linear output is bf16, layers/linear.py:51,73,153; SiluAndMul in fp32 on that, layers/activation.py:8-11).
-First run on a B200 in round 2 (all green); part of the default GPU suite since.
+Part of the default GPU suite.
 """
 import pytest
 import torch

@@ -122,7 +122,7 @@ def test_engine_greedy_generate_vs_oracle(tiny_dir, eager):
 @pytest.mark.parametrize("eager", [True, False])
 def test_engine_two_stream_decode_vs_oracle(tiny_dir, eager, monkeypatch):
     """B200_DUAL=1: every decode step of >= 2 rows runs as two half batches on two streams (event chain between the two
-    attention launches, tcgen05 projections with a 3-slot ring, captured into the decode graphs when not eager); greedy
+    attention launches, wgmma projections with a 3-slot ring, captured into the decode graphs when not eager); greedy
     tokens teacher-forced against the oracle, and equal to the single-stream engine's wherever the oracle has a clear winner."""
     from nanovllm import LLM, SamplingParams
     from nanovllm.utils.synthetic import PRESETS, random_weights

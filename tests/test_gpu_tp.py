@@ -13,7 +13,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 @pytest.mark.parametrize("eager", ["1", "0"])
 def test_tp2_engine_matches_oracle(eager):
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     env = dict(os.environ, TP_EAGER=eager)
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
            "--master-port", str(29555 + int(eager)), os.path.join(ROOT, "tests", "tp_worker.py")]
@@ -24,7 +24,7 @@ def test_tp2_engine_matches_oracle(eager):
 
 def test_tp2_spawned_by_the_engine():
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "tp_spawn_check.py")], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
     assert "SPAWN_RESULT" in r.stdout and '"ok": true' in r.stdout

@@ -1,7 +1,7 @@
 """The product's model code (nanovllm/models/qwen3.py) with every GPU op replaced by a CPU stand-in built from the
 oracle's free functions: checks the PYTHON around the kernels -- which op is called when, with which views, strides,
 argument order and return values -- without a GPU.  On the default path the stand-ins are the oracle's own arithmetic,
-so the logits must equal the oracle's bit for bit; on the tcgen05 paths (B200_LINEAR=tc: tcgen05 projections with fused
+so the logits must equal the oracle's bit for bit; on the wgmma paths (B200_LINEAR=tc: wgmma projections with fused
 SiluAndMul / split-K partial sums) only the summation order differs.
 
 This does not test any kernel (tests/test_gpu_*.py do); it exists so that a typo in the glue of a path that has not
@@ -97,7 +97,7 @@ class CpuOps:
         self._count("store_kv")
         store_kvcache_ref(k, v, self.kv[layer][0], self.kv[layer][1], slot_mapping)
 
-    # ---- tcgen05 projections ----------------------------------------------------------------------------------------
+    # ---- wgmma projections ------------------------------------------------------------------------------------------
     class pdl_off:
         depth = 0
 
@@ -249,8 +249,8 @@ def test_tc_linear_path_glue(preset, monkeypatch):
 
 @pytest.mark.parametrize("preset,fused_max", [("tiny", None), ("tiny", 0)])
 def test_two_stream_decode_path_glue(preset, fused_max, monkeypatch):
-    """B200_DUAL=1: decode batches are cut into two halves (streams on the GPU; plain order here) that each run the tcgen05
-    chain on their own rows / block tables / context lengths; the result must be the single-stream tcgen05 result (only
+    """B200_DUAL=1: decode batches are cut into two halves (streams on the GPU; plain order here) that each run the wgmma
+    chain on their own rows / block tables / context lengths; the result must be the single-stream wgmma result (only
     the split-K summation order differs from the oracle)."""
     got, want, fake, model = run_product_model(monkeypatch, preset, {"B200_DUAL": "1", "B200_DUAL_MIN": "2", "B200_LINEAR": "cublas",
                                                                     "B200_DUAL_CFG": "32,32,64,4,64,4,3"}, fused_decode_max=fused_max)
@@ -269,7 +269,7 @@ def test_two_stream_decode_path_glue(preset, fused_max, monkeypatch):
 
 
 def test_gate_up_only_tc_mode_glue(monkeypatch):
-    """B200_LINEAR=gu: decode steps run gate_up + SiluAndMul as ONE tcgen05 op, every other projection stays a library call
+    """B200_LINEAR=gu: decode steps run gate_up + SiluAndMul as ONE wgmma op, every other projection stays a library call
     (the mode tensor-parallel runs use to save a launch per layer); prefill keeps the two-op path."""
     got, want, fake, model = run_product_model(monkeypatch, "tiny", {"B200_LINEAR": "gu"})
     assert model.tc_gate_up and not model.tc_linear
@@ -329,7 +329,7 @@ def test_fused_lm_head_runner_glue(monkeypatch):
 
 @pytest.mark.parametrize("preset", ["tiny", "tiny-g4"])
 def test_default_auto_linear_policy_glue(preset, monkeypatch):
-    """The default policy (B200_LINEAR=auto): o_proj / down_proj of small batches through the split-K tcgen05 path with the
+    """The default policy (B200_LINEAR=auto): o_proj / down_proj of small batches through the split-K wgmma path with the
     fused add-norm, qkv / gate_up through the library; only the summation order differs from the oracle."""
     monkeypatch.delenv("B200_LINEAR", raising=False)
     got, want, fake, model = run_product_model(monkeypatch, preset, {})
