@@ -1,5 +1,12 @@
 // Context lifetime and KV binding behind include/b200_paged_attn.h.
+#include <atomic>
+
 #include "common.cuh"
+
+// Source of b200_ctx::bind_gen.  Process-wide, so that a binding of a new context (or of a context created after
+// b200_destroy) never reuses the generation of an earlier binding: the tensor maps the tensor-core decode caches per
+// generation (decode_mma.cu) would otherwise describe the earlier cache.
+static std::atomic<uint64_t> g_bind_generation{0};
 
 extern "C" int b200_abi_version(void) { return 2; }
 
@@ -62,6 +69,6 @@ extern "C" int b200_kv_bind(b200_ctx* ctx, void* k_base, void* v_base, int layer
     ctx->block_shift = shift;
     ctx->num_kv_heads = num_kv_heads;
     ctx->head_dim = head_dim;
-    ctx->bind_gen++;
+    ctx->bind_gen = ++g_bind_generation;
     return B200_OK;
 }

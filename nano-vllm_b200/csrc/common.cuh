@@ -23,7 +23,7 @@ struct b200_ctx {
     int num_kv_heads = 0;
     int head_dim = 0;
     std::string last_cuda_error;
-    uint64_t bind_gen = 0;          // bumped by every b200_kv_bind (cached TMA descriptors key on it)
+    uint64_t bind_gen = 0;          // set by every b200_kv_bind, unique within the process (cached TMA descriptors key on it)
 
     size_t layer_elems() const {
         return (size_t)num_blocks * num_kv_heads * block_size * head_dim;
