@@ -72,6 +72,28 @@ int b200_abi_version(void);
 int b200_kv_bind(b200_ctx* ctx, void* k_base, void* v_base, int layers, int64_t num_blocks,
                  int block_size, int num_kv_heads, int head_dim);
 
+/* The same binding over an fp8 (e4m3, OCP "fn" flavour) cache: same layout with 1-byte elements, so the caller allocates
+ * 2 * layers * num_blocks * num_kv_heads * block_size * head_dim bytes.  vLLM's kv_cache_dtype="fp8" (no reference
+ * counterpart).  Every cache write stores e4m3_satfinite_rn(x / scale) of the bf16 value the bf16 binding would store
+ * (k_scale for keys, v_scale for values; out-of-range values saturate to +-448); every read uses float(e4m3) * scale.
+ * Scales must be finite and > 0 (B200_EINVAL otherwise).  On such a binding:
+ *   b200_store_kv, b200_qknorm_rope_store   quantize;
+ *   b200_paged_decode                       runs the tensor-core kernel's fp8 variant for every head group;
+ *   b200_paged_decode_fused                 returns B200_EUNSUPPORTED (use b200_qknorm_rope_store + b200_paged_decode);
+ *   b200_paged_prefill with block_tables    returns B200_EUNSUPPORTED: dequantize with b200_kv_gather and run
+ *                                           b200_prefill_packed_kv on the packed bf16 rows. */
+int b200_kv_bind_fp8(b200_ctx* ctx, void* k_base, void* v_base, int layers, int64_t num_blocks, int block_size,
+                     int num_kv_heads, int head_dim, float k_scale, float v_scale);
+
+/* Dequantizes keys and values 0..len_k(s)-1 of each of num_seqs sequences of an fp8 binding (b200_kv_bind_fp8) into
+ * packed bf16 rows: row r of sequence s goes to k_out / v_out row cu_seqlens_k[s] + r ([total_k, num_kv_heads, head_dim],
+ * row strides in elements), value bf16(float(e4m3) * scale).  len_k(s) = cu_seqlens_k[s+1] - cu_seqlens_k[s]; pages
+ * through block_tables[s] (row stride bt_stride) as b200_paged_prefill reads them.  total_k = cu_seqlens_k[num_seqs].
+ * B200_EUNSUPPORTED on a bf16 binding. */
+int b200_kv_gather(b200_ctx* ctx, int layer, const int32_t* block_tables, int bt_stride, const int32_t* cu_seqlens_k,
+                   int num_seqs, void* k_out, int64_t k_stride0, void* v_out, int64_t v_stride0, int total_k,
+                   void* stream);
+
 /* Bytes of scratch b200_paged_decode needs for batches up to max_batch with num_q_heads query
  * heads.  The caller zero-fills it once (and again after a b200_kv_bind that changes num_kv_heads: the
  * layout depends on it); every launch leaves its counters zeroed. */
@@ -126,6 +148,16 @@ int b200_paged_prefill(b200_ctx* ctx, int layer, const void* q, int64_t q_stride
                        const int32_t* block_tables, int bt_stride, void* out, int64_t out_stride0,
                        int total_q, int num_seqs, int max_seqlen_q, int max_seqlen_k,
                        int num_q_heads, int num_kv_heads, float scale, void* stream);
+
+/* The packed form of b200_paged_prefill (block_tables == NULL) when keys outnumber queries: sequence s attends
+ * len_k(s) = cu_seqlens_k[s+1] - cu_seqlens_k[s] >= len_q(s) keys at rows cu_seqlens_k[s].. of k, v
+ * ([total_k, num_kv_heads, head_dim], total_k = cu_seqlens_k[num_seqs]), same bottom-right aligned causal mask.  This is
+ * the prefix-hit / chunked prefill over an fp8 cache once b200_kv_gather has dequantized its keys and values (in
+ * b200_paged_prefill's packed mode the keys are the step's own rows, so total_k = total_q there). */
+int b200_prefill_packed_kv(b200_ctx* ctx, const void* q, int64_t q_stride0, const void* k, int64_t k_stride0,
+                           const void* v, int64_t v_stride0, const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
+                           void* out, int64_t out_stride0, int total_q, int total_k, int num_seqs, int max_seqlen_q,
+                           int num_q_heads, int num_kv_heads, float scale, void* stream);
 
 /* ---- the fused ops around it (the reference's five @torch.compile sites) ---------------- */
 

@@ -1,5 +1,6 @@
 // Context lifetime and KV binding behind include/b200_paged_attn.h.
 #include <atomic>
+#include <cmath>
 
 #include "common.cuh"
 
@@ -54,8 +55,8 @@ extern "C" int b200_set_pdl(int enabled) {
     return was;
 }
 
-extern "C" int b200_kv_bind(b200_ctx* ctx, void* k_base, void* v_base, int layers,
-                            int64_t num_blocks, int block_size, int num_kv_heads, int head_dim) {
+static int kv_bind(b200_ctx* ctx, void* k_base, void* v_base, int layers, int64_t num_blocks, int block_size,
+                   int num_kv_heads, int head_dim, bool fp8, float k_scale, float v_scale) {
     if (!ctx || !k_base || !v_base || layers <= 0 || num_blocks <= 0 || num_kv_heads <= 0) return B200_EINVAL;
     if (head_dim != B200_HEAD_DIM) return B200_EUNSUPPORTED;
     const int shift = ilog2_exact(block_size);
@@ -69,6 +70,20 @@ extern "C" int b200_kv_bind(b200_ctx* ctx, void* k_base, void* v_base, int layer
     ctx->block_shift = shift;
     ctx->num_kv_heads = num_kv_heads;
     ctx->head_dim = head_dim;
+    ctx->kv_fp8 = fp8;
+    ctx->k_scale = k_scale;
+    ctx->v_scale = v_scale;
     ctx->bind_gen = ++g_bind_generation;
     return B200_OK;
+}
+
+extern "C" int b200_kv_bind(b200_ctx* ctx, void* k_base, void* v_base, int layers,
+                            int64_t num_blocks, int block_size, int num_kv_heads, int head_dim) {
+    return kv_bind(ctx, k_base, v_base, layers, num_blocks, block_size, num_kv_heads, head_dim, false, 1.f, 1.f);
+}
+
+extern "C" int b200_kv_bind_fp8(b200_ctx* ctx, void* k_base, void* v_base, int layers, int64_t num_blocks,
+                                int block_size, int num_kv_heads, int head_dim, float k_scale, float v_scale) {
+    if (!(std::isfinite(k_scale) && k_scale > 0.f) || !(std::isfinite(v_scale) && v_scale > 0.f)) return B200_EINVAL;
+    return kv_bind(ctx, k_base, v_base, layers, num_blocks, block_size, num_kv_heads, head_dim, true, k_scale, v_scale);
 }

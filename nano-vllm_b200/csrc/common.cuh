@@ -2,6 +2,8 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <stdint.h>
 #include <string>
 
@@ -24,12 +26,18 @@ struct b200_ctx {
     int head_dim = 0;
     std::string last_cuda_error;
     uint64_t bind_gen = 0;          // set by every b200_kv_bind, unique within the process (cached TMA descriptors key on it)
+    // b200_kv_bind_fp8: the cache holds e4m3 bytes, element = e4m3_satfinite_rn(x / scale), read back as float(e) * scale.
+    // k_base / v_base then point at bytes: use the *_layer8 accessors, never k_layer / v_layer.
+    bool kv_fp8 = false;
+    float k_scale = 1.f, v_scale = 1.f;
 
     size_t layer_elems() const {
         return (size_t)num_blocks * num_kv_heads * block_size * head_dim;
     }
     __nv_bfloat16* k_layer(int l) const { return k_base + (size_t)l * layer_elems(); }
     __nv_bfloat16* v_layer(int l) const { return v_base + (size_t)l * layer_elems(); }
+    uint8_t* k_layer8(int l) const { return reinterpret_cast<uint8_t*>(k_base) + (size_t)l * layer_elems(); }
+    uint8_t* v_layer8(int l) const { return reinterpret_cast<uint8_t*>(v_base) + (size_t)l * layer_elems(); }
 };
 
 #define B200_CUDA_CHECK(ctx, expr)                                   \
@@ -113,6 +121,27 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
     w.z = pack_bf16x2(f[4], f[5]);
     w.w = pack_bf16x2(f[6], f[7]);
     return w;
+}
+
+// ------------------------------------------------------------------------------------------
+// e4m3 cache elements (b200_kv_bind_fp8).  Quantize: e4m3_satfinite_rn(x / scale), one F2FP per pair (low byte = first
+// element).  Dequantize: every e4m3 value is exact in fp16, so one F2FP per pair gives the exact value.
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t quant4_e4m3(float a, float b, float c, float d, float scale) {
+    const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(a, scale), __fdiv_rn(b, scale)), __NV_SATFINITE, __NV_E4M3);
+    const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(c, scale), __fdiv_rn(d, scale)), __NV_SATFINITE, __NV_E4M3);
+    return lo | (hi << 16);
+}
+// 8 bf16 (one 16-byte word) -> 8 e4m3 (one 8-byte word)
+__device__ __forceinline__ uint2 quant8_e4m3(const uint4& w, float scale) {
+    float f[8];
+    unpack8(w, f);
+    return make_uint2(quant4_e4m3(f[0], f[1], f[2], f[3], scale), quant4_e4m3(f[4], f[5], f[6], f[7], scale));
+}
+// two e4m3 (low byte first) -> f16x2 (low half first)
+__device__ __forceinline__ uint32_t e4m3x2_to_f16x2(uint32_t two) {
+    const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(two & 0xffffu), __NV_E4M3);
+    return (uint32_t)h.x | ((uint32_t)h.y << 16);
 }
 
 // ------------------------------------------------------------------------------------------

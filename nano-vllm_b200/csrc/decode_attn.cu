@@ -496,7 +496,8 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) paged_decode_kernel(const Deco
 
 constexpr int kMaxWarps = 16;   // workspace is sized for the widest variant
 
-// (warps per CTA, ring depth) variants; B200_DECODE_CFG=<warps>x<stages> picks one at first use (tuning knob).
+// (warps per CTA, ring depth) variants; B200_DECODE_CFG=<warps>x<stages> picks one at first use (tuning knob).  Like
+// B200_DECODE and B200_DECODE_L2HINT it chooses among the bf16-cache kernels only: an fp8 cache has one kernel.
 template <int G, int NW, int NS, bool FUSED>
 int launch_variant(b200_ctx* ctx, const DecodeParams& prm, cudaStream_t stream) {
     using L = DecodeSmem<G, NW, NS, FUSED>;
@@ -601,10 +602,14 @@ static int decode_common(b200_ctx* ctx, int layer, const void* q, int64_t q_stri
     prm.q_stride = q_stride0;
     prm.out = static_cast<__nv_bfloat16*>(out);
     prm.out_stride = out_stride0;
-    prm.k_layer = ctx->k_layer(layer);
-    prm.v_layer = ctx->v_layer(layer);
-    prm.k_layer_w = ctx->k_layer(layer);
-    prm.v_layer_w = ctx->v_layer(layer);
+    const bool fp8 = ctx->kv_fp8;
+    prm.k_layer = fp8 ? nullptr : ctx->k_layer(layer);
+    prm.v_layer = fp8 ? nullptr : ctx->v_layer(layer);
+    prm.k_layer_w = fp8 ? nullptr : ctx->k_layer(layer);
+    prm.v_layer_w = fp8 ? nullptr : ctx->v_layer(layer);
+    prm.k8 = fp8 ? ctx->k_layer8(layer) : nullptr;
+    prm.v8 = fp8 ? ctx->v_layer8(layer) : nullptr;
+    prm.v_scale = ctx->v_scale;
     prm.block_tables = block_tables;
     prm.bt_stride = bt_stride;
     prm.context_lens = context_lens;
@@ -612,6 +617,7 @@ static int decode_common(b200_ctx* ctx, int layer, const void* q, int64_t q_stri
     prm.hkv = hkv;
     prm.block_shift = ctx->block_shift;
     prm.scale_log2 = scale * 1.4426950408889634f;
+    if (fp8) prm.scale_log2 *= ctx->k_scale;
     prm.q_norm_w = static_cast<const __nv_bfloat16*>(q_norm_w);
     prm.k_norm_w = static_cast<const __nv_bfloat16*>(k_norm_w);
     prm.cos_sin = cos_sin;
@@ -629,6 +635,11 @@ static int decode_common(b200_ctx* ctx, int layer, const void* q, int64_t q_stri
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // Kernel choice by head-group size (measured on the benchmark's batch-256 step, same KV bytes):
     //   G = 2: FMA 97.6 us, MMA 99.4 us      G = 4: FMA 121.6, MMA 101.9      G = 8: FMA 215.7, MMA 104.2
+    // An fp8 cache always takes the tensor-core kernel's fp8 variant, whatever the head group: 120 us against the bf16
+    // FMA kernel's 204 us on the benchmark's batch-256 step (DESIGN.md 3.5).  An fp8 FMA formulation would need about
+    // twice the ALU work per byte of a kernel that is already near its issue limit, so there is none.  The fused front
+    // end has no quantized KV append.
+    if (fp8) return fused ? B200_EUNSUPPORTED : b200_decode_mma_launch(ctx, layer, prm, G, st);
     if (fused) {
         if (G > 2) return B200_EUNSUPPORTED;
         return G == 1 ? launch_decode<1, true>(ctx, prm, st) : launch_decode<2, true>(ctx, prm, st);

@@ -37,6 +37,10 @@ struct DecodeParams {
     __nv_bfloat16* v_layer_w;
     float eps;
     int l2_hint;                // 1: K/V bulk copies carry an L2 evict_first policy (tuning knob)
+    // fp8 binding (decode_mma.cu's fp8 kernel): the layer's e4m3 K / V bytes; the K scale is already in scale_log2
+    const uint8_t* k8;
+    const uint8_t* v8;
+    float v_scale;
 };
 
 // Walks chunks in (sequence, kv head, chunk) order.  Warp-uniform.

@@ -137,12 +137,19 @@ bool launch_rmsnorm_warp(const __nv_bfloat16* x, int64_t xs, __nv_bfloat16* res,
 // q_norm / k_norm (models/qwen3.py:82-84) + rotary_emb (layers/rotary_embedding.py:37-48) +
 // store_kvcache (layers/attention.py:10-40) over the fused qkv GEMM output.  One HALF-warp per (token, head):
 // lane j owns elements 8j..8j+7 (one 16-byte access), its rotation partner (element +-64) is lane j^8.
-__global__ void __launch_bounds__(128) qknorm_rope_store_kernel(
+// Lane j's 8 elements of one cache row: the bf16 bits as they are, or (fp8 binding) e4m3_satfinite_rn(x / scale).
+template <bool F8>
+__device__ __forceinline__ void store_row_slice(void* cache, int64_t row, int j, const uint4& val, float scale) {
+    if constexpr (F8) reinterpret_cast<uint2*>(static_cast<uint8_t*>(cache) + row * B200_HEAD_DIM)[j] = quant8_e4m3(val, scale);
+    else reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(cache) + row * B200_HEAD_DIM)[j] = val;
+}
+
+template <bool F8>
+__device__ __forceinline__ void qknorm_rope_store_unit(
     __nv_bfloat16* qkv, int64_t stride, int hq, int hkv, const int64_t* __restrict__ positions,
     const __nv_bfloat16* __restrict__ qw, const __nv_bfloat16* __restrict__ kw,
     const float* __restrict__ cos_sin, float eps, const int32_t* __restrict__ slot_mapping,
-    __nv_bfloat16* k_cache, __nv_bfloat16* v_cache, int block_shift, int n) {
-    B200_PDL_SYNC();
+    void* k_cache, void* v_cache, float k_scale, float v_scale, int block_shift, int n) {
     const int heads = hq + 2 * hkv;
     const int64_t unit = ((int64_t)blockIdx.x * 128 + threadIdx.x) >> 4;        // (token, head) index
     const int j = threadIdx.x & 15;
@@ -190,7 +197,7 @@ __global__ void __launch_bounds__(128) qknorm_rope_store_kernel(
     if (is_v) {                                    // a value head: scatter only
         if (slot >= 0) {
             const int kvh = head - hq - hkv;
-            *reinterpret_cast<uint4*>(v_cache + (crow + ((int64_t)kvh << block_shift)) * B200_HEAD_DIM + j * 8) = raw;
+            store_row_slice<F8>(v_cache, crow + ((int64_t)kvh << block_shift), j, raw, v_scale);
         }
         return;
     }
@@ -198,20 +205,40 @@ __global__ void __launch_bounds__(128) qknorm_rope_store_kernel(
     *reinterpret_cast<uint4*>(src) = outv;
     if (!is_q && slot >= 0) {
         const int kvh = head - hq;
-        *reinterpret_cast<uint4*>(k_cache + (crow + ((int64_t)kvh << block_shift)) * B200_HEAD_DIM + j * 8) = outv;
+        store_row_slice<F8>(k_cache, crow + ((int64_t)kvh << block_shift), j, outv, k_scale);
     }
 }
 
-// The same op for prefill-size batches: one HALF-warp per TOKEN walking over its heads.  Lane j owns the same 8 dims of
-// every head, so positions / cos / sin / norm weights / the cache row are fetched once per token instead of once per
-// (token, head), there is no 64-bit division, and U independent 16-byte loads per lane are in flight.
-template <int U>
-__global__ void __launch_bounds__(128) qknorm_rope_store_tok_kernel(
+__global__ void __launch_bounds__(128) qknorm_rope_store_kernel(
     __nv_bfloat16* qkv, int64_t stride, int hq, int hkv, const int64_t* __restrict__ positions,
     const __nv_bfloat16* __restrict__ qw, const __nv_bfloat16* __restrict__ kw,
     const float* __restrict__ cos_sin, float eps, const int32_t* __restrict__ slot_mapping,
     __nv_bfloat16* k_cache, __nv_bfloat16* v_cache, int block_shift, int n) {
     B200_PDL_SYNC();
+    qknorm_rope_store_unit<false>(qkv, stride, hq, hkv, positions, qw, kw, cos_sin, eps, slot_mapping, k_cache, v_cache,
+                                  1.f, 1.f, block_shift, n);
+}
+
+// the same op over an fp8 binding (one kernel per cache dtype, so the profiler names which one ran)
+__global__ void __launch_bounds__(128) qknorm_rope_store_fp8_kernel(
+    __nv_bfloat16* qkv, int64_t stride, int hq, int hkv, const int64_t* __restrict__ positions,
+    const __nv_bfloat16* __restrict__ qw, const __nv_bfloat16* __restrict__ kw,
+    const float* __restrict__ cos_sin, float eps, const int32_t* __restrict__ slot_mapping,
+    uint8_t* k_cache, uint8_t* v_cache, float k_scale, float v_scale, int block_shift, int n) {
+    B200_PDL_SYNC();
+    qknorm_rope_store_unit<true>(qkv, stride, hq, hkv, positions, qw, kw, cos_sin, eps, slot_mapping, k_cache, v_cache,
+                                 k_scale, v_scale, block_shift, n);
+}
+
+// The same op for prefill-size batches: one HALF-warp per TOKEN walking over its heads.  Lane j owns the same 8 dims of
+// every head, so positions / cos / sin / norm weights / the cache row are fetched once per token instead of once per
+// (token, head), there is no 64-bit division, and U independent 16-byte loads per lane are in flight.
+template <int U, bool F8>
+__device__ __forceinline__ void qknorm_rope_store_token(
+    __nv_bfloat16* qkv, int64_t stride, int hq, int hkv, const int64_t* __restrict__ positions,
+    const __nv_bfloat16* __restrict__ qw, const __nv_bfloat16* __restrict__ kw,
+    const float* __restrict__ cos_sin, float eps, const int32_t* __restrict__ slot_mapping,
+    void* k_cache, void* v_cache, float k_scale, float v_scale, int block_shift, int n) {
     const int heads = hq + 2 * hkv;
     const int t_raw = blockIdx.x * 8 + (threadIdx.x >> 4);
     const bool live = t_raw < n;                       // a dead half-warp still takes part in the full-warp shuffles
@@ -243,7 +270,7 @@ __global__ void __launch_bounds__(128) qknorm_rope_store_tok_kernel(
             if (head >= heads) break;                  // uniform across the warp
             if (head >= hq + hkv) {                    // a value head: scatter only
                 if (live && slot >= 0)
-                    *reinterpret_cast<uint4*>(v_cache + (crow + ((int64_t)(head - hq - hkv) << block_shift)) * B200_HEAD_DIM + j * 8) = raw[u];
+                    store_row_slice<F8>(v_cache, crow + ((int64_t)(head - hq - hkv) << block_shift), j, raw[u], v_scale);
                 continue;
             }
             const bool is_q = head < hq;
@@ -267,10 +294,32 @@ __global__ void __launch_bounds__(128) qknorm_rope_store_tok_kernel(
                 const uint4 outv = pack8(y);
                 *reinterpret_cast<uint4*>(row + head * B200_HEAD_DIM) = outv;
                 if (!is_q && slot >= 0)
-                    *reinterpret_cast<uint4*>(k_cache + (crow + ((int64_t)(head - hq) << block_shift)) * B200_HEAD_DIM + j * 8) = outv;
+                    store_row_slice<F8>(k_cache, crow + ((int64_t)(head - hq) << block_shift), j, outv, k_scale);
             }
         }
     }
+}
+
+template <int U>
+__global__ void __launch_bounds__(128) qknorm_rope_store_tok_kernel(
+    __nv_bfloat16* qkv, int64_t stride, int hq, int hkv, const int64_t* __restrict__ positions,
+    const __nv_bfloat16* __restrict__ qw, const __nv_bfloat16* __restrict__ kw,
+    const float* __restrict__ cos_sin, float eps, const int32_t* __restrict__ slot_mapping,
+    __nv_bfloat16* k_cache, __nv_bfloat16* v_cache, int block_shift, int n) {
+    B200_PDL_SYNC();
+    qknorm_rope_store_token<U, false>(qkv, stride, hq, hkv, positions, qw, kw, cos_sin, eps, slot_mapping, k_cache, v_cache,
+                                      1.f, 1.f, block_shift, n);
+}
+
+template <int U>
+__global__ void __launch_bounds__(128) qknorm_rope_store_tok_fp8_kernel(
+    __nv_bfloat16* qkv, int64_t stride, int hq, int hkv, const int64_t* __restrict__ positions,
+    const __nv_bfloat16* __restrict__ qw, const __nv_bfloat16* __restrict__ kw,
+    const float* __restrict__ cos_sin, float eps, const int32_t* __restrict__ slot_mapping,
+    uint8_t* k_cache, uint8_t* v_cache, float k_scale, float v_scale, int block_shift, int n) {
+    B200_PDL_SYNC();
+    qknorm_rope_store_token<U, true>(qkv, stride, hq, hkv, positions, qw, kw, cos_sin, eps, slot_mapping, k_cache, v_cache,
+                                     k_scale, v_scale, block_shift, n);
 }
 
 // store_kvcache_kernel (layers/attention.py:10-30): one warp per (token, kv head).
@@ -292,6 +341,69 @@ __global__ void __launch_bounds__(128) store_kv_kernel(const __nv_bfloat16* __re
         reinterpret_cast<const uint2*>(k + (int64_t)tok * k_stride + kvh * B200_HEAD_DIM)[lane];
     reinterpret_cast<uint2*>(v_cache + row * B200_HEAD_DIM)[lane] =
         reinterpret_cast<const uint2*>(v + (int64_t)tok * v_stride + kvh * B200_HEAD_DIM)[lane];
+}
+
+// store_kv_kernel over an fp8 binding: lane i quantizes elements 4i..4i+3 of the row.
+__global__ void __launch_bounds__(128) store_kv_fp8_kernel(const __nv_bfloat16* __restrict__ k, int64_t k_stride,
+                                                           const __nv_bfloat16* __restrict__ v, int64_t v_stride,
+                                                           const int32_t* __restrict__ slot_mapping, uint8_t* k_cache,
+                                                           uint8_t* v_cache, float k_scale, float v_scale, int hkv,
+                                                           int block_shift, int n) {
+    B200_PDL_SYNC();
+    const int64_t gwarp = (int64_t)blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (gwarp >= (int64_t)n * hkv) return;
+    const int tok = (int)(gwarp / hkv);
+    const int kvh = (int)(gwarp - (int64_t)tok * hkv);
+    const int lane = threadIdx.x & 31;
+    const int slot = slot_mapping[tok];
+    if (slot < 0) return;
+    const int64_t row = ((((int64_t)(slot >> block_shift)) * hkv + kvh) << block_shift) + (slot & ((1 << block_shift) - 1));
+    const uint2 kw = reinterpret_cast<const uint2*>(k + (int64_t)tok * k_stride + kvh * B200_HEAD_DIM)[lane];
+    const uint2 vw = reinterpret_cast<const uint2*>(v + (int64_t)tok * v_stride + kvh * B200_HEAD_DIM)[lane];
+    reinterpret_cast<uint32_t*>(k_cache + row * B200_HEAD_DIM)[lane] =
+        quant4_e4m3(bf16lo(kw.x), bf16hi(kw.x), bf16lo(kw.y), bf16hi(kw.y), k_scale);
+    reinterpret_cast<uint32_t*>(v_cache + row * B200_HEAD_DIM)[lane] =
+        quant4_e4m3(bf16lo(vw.x), bf16hi(vw.x), bf16lo(vw.y), bf16hi(vw.y), v_scale);
+}
+
+// Dequantize rows 0..len_k(s)-1 of every sequence s of an fp8 binding into packed bf16 [total_k, hkv, 128]
+// (row r of sequence s at cu_k[s] + r): one warp per packed row, lane j of a half-warp owns 8 dims of a head.
+__global__ void __launch_bounds__(128) kv_gather_fp8_kernel(const uint8_t* __restrict__ k_cache, const uint8_t* __restrict__ v_cache,
+                                                            const int32_t* __restrict__ block_tables, int bt_stride,
+                                                            const int32_t* __restrict__ cu_k, int num_seqs,
+                                                            __nv_bfloat16* k_out, int64_t k_stride, __nv_bfloat16* v_out,
+                                                            int64_t v_stride, float k_scale, float v_scale, int hkv,
+                                                            int block_shift, int total_k) {
+    B200_PDL_SYNC();
+    const int r = blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (r >= total_k) return;
+    const int lane = threadIdx.x & 31;
+    int lo = 0, hi = num_seqs;                          // the sequence s with cu_k[s] <= r < cu_k[s + 1]
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (cu_k[mid] <= r) lo = mid; else hi = mid;
+    }
+    const int t = r - cu_k[lo];
+    const int page = block_tables[(int64_t)lo * bt_stride + (t >> block_shift)];
+    const int64_t row0 = ((int64_t)page * hkv << block_shift) + (t & ((1 << block_shift) - 1));
+    for (int u = lane; u < hkv * 16; u += 32) {
+        const int h = u >> 4, j = u & 15;
+        const int64_t crow = row0 + ((int64_t)h << block_shift);
+        const uint2 kq = reinterpret_cast<const uint2*>(k_cache + crow * B200_HEAD_DIM)[j];
+        const uint2 vq = reinterpret_cast<const uint2*>(v_cache + crow * B200_HEAD_DIM)[j];
+        float kf[8], vf[8];
+        const uint32_t kw[4] = {kq.x, kq.x >> 16, kq.y, kq.y >> 16}, vw[4] = {vq.x, vq.x >> 16, vq.y, vq.y >> 16};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const uint32_t hk = e4m3x2_to_f16x2(kw[e]), hv = e4m3x2_to_f16x2(vw[e]);
+            const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&hk));
+            const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&hv));
+            kf[2 * e] = a.x * k_scale; kf[2 * e + 1] = a.y * k_scale;
+            vf[2 * e] = b.x * v_scale; vf[2 * e + 1] = b.y * v_scale;
+        }
+        reinterpret_cast<uint4*>(k_out + (int64_t)r * k_stride + h * B200_HEAD_DIM)[j] = pack8(kf);
+        reinterpret_cast<uint4*>(v_out + (int64_t)r * v_stride + h * B200_HEAD_DIM)[j] = pack8(vf);
+    }
 }
 
 // SiluAndMul.forward (layers/activation.py:8-11)
@@ -381,13 +493,29 @@ extern "C" int b200_qknorm_rope_store(b200_ctx* ctx, int layer, void* qkv, int64
     if (n == 0) return B200_OK;
     __nv_bfloat16 *kc = nullptr, *vc = nullptr;
     int shift = 0;
+    const bool fp8 = slot_mapping != nullptr && ctx->k_base != nullptr && ctx->kv_fp8;
     if (slot_mapping != nullptr && ctx->k_base != nullptr) {
         if (layer < 0 || layer >= ctx->layers || num_kv_heads != ctx->num_kv_heads) return B200_EINVAL;
-        kc = ctx->k_layer(layer);
-        vc = ctx->v_layer(layer);
+        if (!fp8) {
+            kc = ctx->k_layer(layer);
+            vc = ctx->v_layer(layer);
+        }
         shift = ctx->block_shift;
     }
     static const int tok_min = [] { const char* e = getenv("B200_QKNORM_TOK_MIN"); return e ? atoi(e) : 2048; }();
+    if (fp8) {
+        if (n >= tok_min)
+            B200_LAUNCH((qknorm_rope_store_tok_fp8_kernel<8>), (unsigned)((n + 7) / 8), 128, 0, static_cast<cudaStream_t>(stream),
+                static_cast<__nv_bfloat16*>(qkv), qkv_stride0, num_q_heads, num_kv_heads, positions,
+                static_cast<const __nv_bfloat16*>(q_norm_weight), static_cast<const __nv_bfloat16*>(k_norm_weight),
+                cos_sin, eps, slot_mapping, ctx->k_layer8(layer), ctx->v_layer8(layer), ctx->k_scale, ctx->v_scale, shift, n);
+        else
+            B200_LAUNCH((qknorm_rope_store_fp8_kernel), (unsigned)(((int64_t)n * (num_q_heads + 2 * num_kv_heads) + 7) / 8), 128, 0,
+                static_cast<cudaStream_t>(stream), static_cast<__nv_bfloat16*>(qkv), qkv_stride0, num_q_heads, num_kv_heads,
+                positions, static_cast<const __nv_bfloat16*>(q_norm_weight), static_cast<const __nv_bfloat16*>(k_norm_weight),
+                cos_sin, eps, slot_mapping, ctx->k_layer8(layer), ctx->v_layer8(layer), ctx->k_scale, ctx->v_scale, shift, n);
+        return b200_launch_status(ctx);
+    }
     if (n >= tok_min) {             // prefill-size batch: one half-warp per token (see the kernel)
         B200_LAUNCH((qknorm_rope_store_tok_kernel<8>), (unsigned)((n + 7) / 8), 128, 0, static_cast<cudaStream_t>(stream),
             static_cast<__nv_bfloat16*>(qkv), qkv_stride0, num_q_heads, num_kv_heads, positions,
@@ -413,9 +541,31 @@ extern "C" int b200_store_kv(b200_ctx* ctx, int layer, const void* k, int64_t k_
     if (k_stride0 % 4 || v_stride0 % 4 || ((uintptr_t)k & 7) || ((uintptr_t)v & 7)) return B200_EINVAL;
     if (n == 0) return B200_OK;
     const int64_t warps = (int64_t)n * ctx->num_kv_heads;
+    if (ctx->kv_fp8) {
+        B200_LAUNCH((store_kv_fp8_kernel), (unsigned)((warps + 3) / 4), 128, 0, static_cast<cudaStream_t>(stream),
+            static_cast<const __nv_bfloat16*>(k), k_stride0, static_cast<const __nv_bfloat16*>(v), v_stride0, slot_mapping,
+            ctx->k_layer8(layer), ctx->v_layer8(layer), ctx->k_scale, ctx->v_scale, ctx->num_kv_heads, ctx->block_shift, n);
+        return b200_launch_status(ctx);
+    }
     B200_LAUNCH((store_kv_kernel), (unsigned)((warps + 3) / 4), 128, 0, static_cast<cudaStream_t>(stream), 
         static_cast<const __nv_bfloat16*>(k), k_stride0, static_cast<const __nv_bfloat16*>(v), v_stride0,
         slot_mapping, ctx->k_layer(layer), ctx->v_layer(layer), ctx->num_kv_heads, ctx->block_shift, n);
+    return b200_launch_status(ctx);
+}
+
+extern "C" int b200_kv_gather(b200_ctx* ctx, int layer, const int32_t* block_tables, int bt_stride,
+                              const int32_t* cu_seqlens_k, int num_seqs, void* k_out, int64_t k_stride0, void* v_out,
+                              int64_t v_stride0, int total_k, void* stream) {
+    if (!ctx || !block_tables || !cu_seqlens_k || !k_out || !v_out || num_seqs < 0 || total_k < 0) return B200_EINVAL;
+    if (!ctx->k_base) return B200_ENOTBOUND;
+    if (!ctx->kv_fp8) return B200_EUNSUPPORTED;
+    if (layer < 0 || layer >= ctx->layers) return B200_EINVAL;
+    if (k_stride0 % 8 || v_stride0 % 8 || !aligned16(k_out) || !aligned16(v_out)) return B200_EINVAL;
+    if (total_k == 0 || num_seqs == 0) return B200_OK;
+    B200_LAUNCH((kv_gather_fp8_kernel), (unsigned)((total_k + 3) / 4), 128, 0, static_cast<cudaStream_t>(stream),
+        ctx->k_layer8(layer), ctx->v_layer8(layer), block_tables, bt_stride, cu_seqlens_k, num_seqs,
+        static_cast<__nv_bfloat16*>(k_out), k_stride0, static_cast<__nv_bfloat16*>(v_out), v_stride0, ctx->k_scale,
+        ctx->v_scale, ctx->num_kv_heads, ctx->block_shift, total_k);
     return b200_launch_status(ctx);
 }
 

@@ -271,13 +271,13 @@ prefill_ws_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
 
 }  // namespace
 
-// Called from b200_paged_prefill (prefill_attn.cu).  Returns B200_EUNSUPPORTED if TMA descriptors cannot be built.
+// Called from b200_paged_prefill / b200_prefill_packed_kv (prefill_attn.cu).  Returns B200_EUNSUPPORTED if TMA descriptors
+// cannot be built.
 int b200_prefill_ws_launch(b200_ctx* ctx, int layer, const void* q, int64_t q_stride0, const void* k, int64_t k_stride0,
                            const void* v, int64_t v_stride0, const int32_t* cu_q, const int32_t* cu_k,
-                           const int32_t* block_tables, int bt_stride, void* out, int64_t out_stride0, int total_q,
+                           const int32_t* block_tables, int bt_stride, void* out, int64_t out_stride0, int total_q, int total_k,
                            int num_seqs, int max_seqlen_q, int num_q_heads, int num_kv_heads, float scale,
                            cudaStream_t stream) {
-    const int total_k = total_q;
     if ((out_stride0 % 8) || ((uintptr_t)out & 15)) return B200_EINVAL;
     CUtensorMap tq, tk, tv;
     if (!make_map(&tq, q, (uint64_t)num_q_heads * D, (uint64_t)total_q, (uint64_t)q_stride0, BM)) return B200_EUNSUPPORTED;

@@ -22,12 +22,15 @@ SIGNATURES = {
     "b200_abi_version": (_i, []),
     "b200_set_pdl": (_i, [_i]),
     "b200_kv_bind": (_i, [_vp, _vp, _vp, _i, _i64, _i, _i, _i]),
+    "b200_kv_bind_fp8": (_i, [_vp, _vp, _vp, _i, _i64, _i, _i, _i, _f, _f]),
+    "b200_kv_gather": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i64, _vp, _i64, _i, _vp]),
     "b200_decode_workspace_bytes": (_sz, [_vp, _i, _i]),
     "b200_store_kv": (_i, [_vp, _i, _vp, _i64, _vp, _i64, _vp, _i, _vp]),
     "b200_paged_decode": (_i, [_vp, _i, _vp, _i64, _vp, _i, _vp, _vp, _i64, _i, _i, _f, _vp, _sz, _vp]),
     "b200_paged_decode_fused": (_i, [_vp, _i, _vp, _i64, _vp, _vp, _vp, _f, _vp, _i, _vp, _vp, _i64, _i, _i, _f, _vp, _sz, _vp]),
     "b200_paged_prefill": (_i, [_vp, _i, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _i, _vp, _i64,
                                  _i, _i, _i, _i, _i, _i, _f, _vp]),
+    "b200_prefill_packed_kv": (_i, [_vp, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _i, _f, _vp]),
     "b200_rmsnorm": (_i, [_vp, _i64, _vp, _vp, _i64, _i, _i, _f, _vp]),
     "b200_add_rmsnorm": (_i, [_vp, _vp, _vp, _vp, _i, _i, _f, _vp]),
     "b200_qknorm_rope_store": (_i, [_vp, _i, _vp, _i64, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _i, _vp]),

@@ -29,7 +29,8 @@ import torch.distributed as dist
 
 from .. import _native as nat
 from .. import ops
-from ..config import Config
+from ..config import KV_CACHE_DTYPES, Config
+from ..layers.attention import KVGroup, kv_group_arrays, plan_kv_groups
 from ..models.qwen3 import Qwen3ForCausalLM
 from ..utils.context import reset_context, set_context
 from ..utils.loader import load_model
@@ -70,6 +71,11 @@ class ModelRunner:
         self.config = config
         hf = config.hf_config
         self.block_size = config.kvcache_block_size
+        self.kv_fp8 = KV_CACHE_DTYPES[config.kv_cache_dtype]
+        # fp8 cache: rows of the bf16 scratch a paged prefill dequantizes keys / values into (one step's new tokens plus
+        # the longest context fit, so one sequence always does; a step that needs more is cut into groups)
+        self.kv_scratch_rows = config.max_num_batched_tokens + config.max_model_len
+        self.kv_scratch = None
         self.enforce_eager = config.enforce_eager
         self.world_size = config.tensor_parallel_size
         self.rank = rank
@@ -180,6 +186,8 @@ class ModelRunner:
             o = _align(o + count * size)
         self.d_bytes = o
         prefill_bytes = _align(8) + 2 * _align(T * 8) + _align(T * 4) + 2 * _align((S + 1) * 4) + _align(S * 4) + _align(S * W * 4)
+        if self.kv_fp8:                                      # the rebased cu_seqlens_q/k of at most S gather groups
+            prefill_bytes += 2 * (8 * S + _ALIGN * S)
         self.stage = _Staging(self.d_bytes, hosts=2)         # ping-pong: step N+1 is staged while step N runs
         self.pstage = _Staging(prefill_bytes)
         st = self.stage
@@ -224,7 +232,12 @@ class ModelRunner:
 
     def kv_block_bytes(self) -> int:
         hf = self.config.hf_config
-        return 2 * hf.num_hidden_layers * self.block_size * self.model.num_kv_heads * self.model.head_dim * 2
+        elem = 1 if self.kv_fp8 else 2
+        return 2 * hf.num_hidden_layers * self.block_size * self.model.num_kv_heads * self.model.head_dim * elem
+
+    def kv_scratch_bytes(self) -> int:
+        """The fp8 cache's dequantization scratch (K and V, bf16); 0 for a bf16 cache."""
+        return 2 * self.kv_scratch_rows * self.model.num_kv_heads * self.model.head_dim * 2 if self.kv_fp8 else 0
 
     def allocate_kv_cache(self):
         """Size the cache from free memory with the reference's formula (model_runner.py:103-113), allocate
@@ -236,7 +249,7 @@ class ModelRunner:
             used = total - free
             stats = torch.cuda.memory_stats()
             peak, current = stats["allocated_bytes.all.peak"], stats["allocated_bytes.all.current"]
-            nblk = int(total * cfg.gpu_memory_utilization - used - peak + current) // self.kv_block_bytes()
+            nblk = int(total * cfg.gpu_memory_utilization - used - peak + current - self.kv_scratch_bytes()) // self.kv_block_bytes()
             if self.world_size > 1:                      # replicas must agree on the block count
                 t = torch.tensor([nblk], dtype=torch.int64, device="cuda")
                 dist.all_reduce(t, op=dist.ReduceOp.MIN)
@@ -245,8 +258,14 @@ class ModelRunner:
         if cfg.num_kvcache_blocks <= 0:
             raise RuntimeError("not enough GPU memory for a single KV-cache block")
         m = self.model
-        self.kv_cache = torch.zeros(ops.kv_cache_shape(hf.num_hidden_layers, cfg.num_kvcache_blocks, m.num_kv_heads,
-                                                       self.block_size, m.head_dim), dtype=torch.bfloat16, device="cuda")
+        shape = ops.kv_cache_shape(hf.num_hidden_layers, cfg.num_kvcache_blocks, m.num_kv_heads, self.block_size, m.head_dim)
+        self.kv_scratch = None
+        if self.kv_fp8:
+            self.kv_cache = torch.zeros(shape, dtype=torch.uint8, device="cuda").view(torch.float8_e4m3fn)
+            self.kv_scratch = torch.empty(2, self.kv_scratch_rows, m.num_kv_heads, m.head_dim, dtype=torch.bfloat16, device="cuda")
+            m.fused_decode_max_batch = 0             # the fused decode front end has no quantized KV append
+        else:
+            self.kv_cache = torch.zeros(shape, dtype=torch.bfloat16, device="cuda")
         ops.bind_kv_cache(self.kv_cache)
         ops.ensure_workspace(self.cap_bs, m.num_heads)
         layer_id = 0
@@ -255,6 +274,7 @@ class ModelRunner:
                 module.k_cache = self.kv_cache[0, layer_id]
                 module.v_cache = self.kv_cache[1, layer_id]
                 module.layer_id = layer_id
+                module.kv_scratch = self.kv_scratch
                 layer_id += 1
 
     # ---- step marshalling (host integer work; must match the reference bit for bit) ------------
@@ -317,8 +337,14 @@ class ModelRunner:
                 ("slot_mapping", a["slot_mapping"], torch.int32),
                 ("cu_seqlens_q", a["cu_seqlens_q"], torch.int32), ("cu_seqlens_k", a["cu_seqlens_k"], torch.int32),
                 ("temps", np.fromiter((s.temperature for s in seqs), dtype=np.float32, count=len(seqs)), torch.float32)]
+        groups = None
         if a["block_tables"] is not None:
             plan.append(("block_tables", np.ascontiguousarray(a["block_tables"]).reshape(-1), torch.int32))
+            if self.kv_fp8 and self.kv_scratch is not None:
+                groups = kv_group_arrays(a["cu_seqlens_q"], a["cu_seqlens_k"],
+                                         plan_kv_groups(a["cu_seqlens_k"], self.kv_scratch_rows))
+                for i, g in enumerate(groups):
+                    plan += [(f"g{i}q", g[6], torch.int32), (f"g{i}k", g[7], torch.int32)]
         for name, arr, tdt in plan:
             h, d = st.views(off, arr.size, arr.dtype, tdt)
             h[:] = arr
@@ -330,8 +356,11 @@ class ModelRunner:
         if bt is not None:
             bt = bt.view(len(seqs), -1)
         slot = views["slot_mapping"] if a["slot_mapping"].size else None
+        kv_groups = None
+        if groups is not None:
+            kv_groups = [KVGroup(*g[:6], views[f"g{i}q"], views[f"g{i}k"]) for i, g in enumerate(groups)]
         set_context(True, views["cu_seqlens_q"], views["cu_seqlens_k"], a["max_seqlen_q"], a["max_seqlen_k"],
-                    slot, None, bt)
+                    slot, None, bt, kv_groups)
         return views["input_ids"], views["positions"], views["temps"], views["step"]
 
     def _padded_rows(self, n: int) -> int:

@@ -39,13 +39,23 @@ def kv_cache_shape(layers, num_blocks, num_kv_heads, block_size, head_dim):
     return (2, layers, num_blocks, num_kv_heads, block_size, head_dim)
 
 
-def bind_kv_cache(kv_cache: torch.Tensor):
-    """kv_cache: [2, L, nblk, Hkv, bs, D] bf16 contiguous (engine/model_runner.py:103-121 equivalent)."""
-    _need(kv_cache, torch.bfloat16, "kv_cache")
+def bind_kv_cache(kv_cache: torch.Tensor, k_scale: float = 1.0, v_scale: float = 1.0):
+    """kv_cache: [2, L, nblk, Hkv, bs, D] bf16 or float8_e4m3fn contiguous (engine/model_runner.py:103-121 equivalent).
+    An fp8 cache stores e4m3(x / scale) and reads e4m3 * scale, k_scale for keys and v_scale for values."""
+    if kv_cache.dtype != torch.float8_e4m3fn:
+        _need(kv_cache, torch.bfloat16, "kv_cache")
+        if k_scale != 1.0 or v_scale != 1.0:
+            raise nat.B200Error("k_scale / v_scale apply to an fp8 (float8_e4m3fn) cache only")
+    elif not kv_cache.is_cuda:
+        raise nat.B200Error("kv_cache must be a CUDA tensor (there is no CPU path)")
     assert kv_cache.is_contiguous() and kv_cache.dim() == 6 and kv_cache.shape[0] == 2
     h = nat.handle()
     _, layers, nblk, hkv, bs, d = kv_cache.shape
-    nat.check(h.lib.b200_kv_bind(h.ptr, kv_cache[0].data_ptr(), kv_cache[1].data_ptr(), layers, nblk, bs, hkv, d), h.ptr)
+    if kv_cache.dtype == torch.float8_e4m3fn:
+        nat.check(h.lib.b200_kv_bind_fp8(h.ptr, kv_cache[0].data_ptr(), kv_cache[1].data_ptr(), layers, nblk, bs, hkv, d,
+                                         k_scale, v_scale), h.ptr)
+    else:
+        nat.check(h.lib.b200_kv_bind(h.ptr, kv_cache[0].data_ptr(), kv_cache[1].data_ptr(), layers, nblk, bs, hkv, d), h.ptr)
     h.kv = kv_cache
     h.workspace = None          # its layout depends on the head count: start again from zeros
     return h
@@ -70,6 +80,21 @@ def store_kv(layer: int, k: torch.Tensor, v: torch.Tensor, slot_mapping: torch.T
     h = nat.handle()
     nat.check(h.lib.b200_store_kv(h.ptr, layer, k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
                                   slot_mapping.data_ptr(), n, _stream()), h.ptr)
+
+
+def kv_gather(layer: int, block_tables: torch.Tensor, cu_seqlens_k: torch.Tensor, k_out: torch.Tensor, v_out: torch.Tensor,
+              total_k: int) -> None:
+    """Dequantize keys / values 0..len_k(s)-1 of every sequence of the bound fp8 cache into packed bf16 rows
+    k_out / v_out [>= total_k, Hkv, D] (row cu_seqlens_k[s] + r for row r of sequence s)."""
+    _need(block_tables, torch.int32, "block_tables"); _need(cu_seqlens_k, torch.int32, "cu_seqlens_k")
+    _need(k_out, torch.bfloat16, "k_out"); _need(v_out, torch.bfloat16, "v_out")
+    d = k_out.shape[-1]
+    assert block_tables.stride(1) == 1 and k_out.stride(2) == 1 and k_out.stride(1) == d and v_out.stride(2) == 1 and v_out.stride(1) == d
+    assert k_out.shape[0] >= total_k and v_out.shape[0] >= total_k
+    h = nat.handle()
+    nat.check(h.lib.b200_kv_gather(h.ptr, layer, block_tables.data_ptr(), block_tables.stride(0), cu_seqlens_k.data_ptr(),
+                                   cu_seqlens_k.numel() - 1, k_out.data_ptr(), k_out.stride(0), v_out.data_ptr(), v_out.stride(0),
+                                   int(total_k), _stream()), h.ptr)
 
 
 def paged_decode(layer: int, q: torch.Tensor, block_tables: torch.Tensor, context_lens: torch.Tensor,
@@ -131,6 +156,25 @@ def paged_prefill(layer: int, q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q:
                                        cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), btp, bts,
                                        out.data_ptr(), out.stride(0), t, cu_seqlens_q.numel() - 1,
                                        int(max_seqlen_q), int(max_seqlen_k), hq, hkv, scale, _stream()), h.ptr)
+    return out
+
+
+def prefill_packed_kv(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q: int, scale: float, out=None) -> torch.Tensor:
+    """Packed causal varlen prefill where sequence s has len_k(s) >= len_q(s) keys: q [T, Hq, D], k / v [Tk, Hkv, D]
+    (all Tk rows are keys: Tk = cu_seqlens_k[-1])."""
+    for t, name in ((q, "q"), (k, "k"), (v, "v")):
+        _need(t, torch.bfloat16, name)
+    _need(cu_seqlens_q, torch.int32, "cu_seqlens_q"); _need(cu_seqlens_k, torch.int32, "cu_seqlens_k")
+    t, hq, d = q.shape
+    hkv = k.shape[1]
+    assert q.stride(2) == 1 and q.stride(1) == d
+    assert k.stride(2) == 1 and k.stride(1) == d and v.stride(2) == 1 and v.stride(1) == d and v.shape[0] == k.shape[0]
+    if out is None:
+        out = torch.empty((t, hq, d), dtype=q.dtype, device=q.device)
+    h = nat.handle()
+    nat.check(h.lib.b200_prefill_packed_kv(h.ptr, q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
+                                           cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), out.data_ptr(), out.stride(0), t,
+                                           k.shape[0], cu_seqlens_q.numel() - 1, int(max_seqlen_q), hq, hkv, scale, _stream()), h.ptr)
     return out
 
 

@@ -12,12 +12,14 @@ Field meaning (shapes as built by the runner, engine/model_runner.py:129-188 in 
   slot_mapping    int32   [T] cache slot of every new token, -1 = skip
   context_lens    int32   [B] keys visible to each decode row, 0 = CUDA-graph padding row
   block_tables    int32   [S or B, W] page ids, -1 padded; None = packed prefill without cache reads
+  kv_groups       list    fp8 cache only: the paged prefill's sequences cut into groups whose keys fit the
+                          dequantization scratch (layers/attention.py:KVGroup); None otherwise
 """
 from __future__ import annotations
 
 _FIELDS = ("is_prefill", "cu_seqlens_q", "cu_seqlens_k", "max_seqlen_q", "max_seqlen_k",
-           "slot_mapping", "context_lens", "block_tables")
-_DEFAULTS = (False, None, None, 0, 0, None, None, None)
+           "slot_mapping", "context_lens", "block_tables", "kv_groups")
+_DEFAULTS = (False, None, None, 0, 0, None, None, None, None)
 
 
 class Context:
@@ -46,9 +48,9 @@ def get_context() -> Context:
 
 
 def set_context(is_prefill, cu_seqlens_q=None, cu_seqlens_k=None, max_seqlen_q=0, max_seqlen_k=0,
-                slot_mapping=None, context_lens=None, block_tables=None) -> None:
+                slot_mapping=None, context_lens=None, block_tables=None, kv_groups=None) -> None:
     _STEP.assign(is_prefill, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k,
-                 slot_mapping, context_lens, block_tables)
+                 slot_mapping, context_lens, block_tables, kv_groups)
 
 
 def reset_context() -> None:
