@@ -243,6 +243,40 @@ int b200_sample(const void* logits, int logits_is_fp32, int64_t logits_stride0,
                 uint64_t seed, uint64_t step, const int64_t* step_dev, int64_t* out,
                 int64_t* out_keys, void* stream);
 
+/* Top-k / top-p / min-p sampling (vLLM v1 semantics; the reference samples the full softmax only), bf16 logits only.
+ * Per row r, with t = temperatures[r] and probabilities those of logits / t:
+ *   top_k[r]  <= 0 or >= vocab: off;  else keep x_j >= the k-th largest logit (ties at the boundary kept)
+ *   top_p[r]  >= 1: off;  else keep x_j iff the mass of the tokens with a strictly larger logit is < top_p[r] times
+ *             the mass that survives top-k and min-p (ties at the boundary kept)
+ *   min_p[r]  <= 0: off;  else keep x_j iff prob_j >= min_p[r] * prob_max
+ * top_k / top_p / min_p may each be NULL (off for every row).  The kept set is {j : x_j >= tau} for one bf16 tau per
+ * row, and the token is b200_sample's exponential race (same RNG, same keys) restricted to it.  Rows with t == 0
+ * (greedy) or every filter off get exactly b200_sample's token.
+ *
+ * Call b200_sample_filter_stage with stage = 0, 1, 2, 3, then b200_sample_filtered, all on the same rows, logits and
+ * workspace.  workspace: b200_sample_filter_workspace_words(rows) int64 words, zero before its first use; the last call
+ * leaves it zero again except for the tau words.  Row r owns words [r * 1538, (r + 1) * 1538):
+ *   word 0             written by stage 0, reduce with MAX: order-preserving key of the row maximum
+ *   word 1             written by b200_sample_filtered: key of tau (bf16 bits b -> b ^ (b & 0x8000 ? 0xffff : 0x8000),
+ *                      -0 as +0); every x with key(x) >= tau is kept.  Not part of any stage.
+ *   words 2..513       written by stage 1, reduce with SUM (256 counts, then 256 fixed-point masses)
+ *   words 514..1025    written by stage 2, reduce with SUM (same form)
+ *   words 1026..1537   written by stage 3, reduce with SUM (same form)
+ * Vocab-parallel use: each rank runs every stage on its shard and all-reduces that stage's words over the ranks before
+ * the next call (every rank launches every stage, whatever its rows need); b200_sample_filtered then takes index_offset
+ * and out_keys as b200_sample does, and one all-reduce(MAX) of out_keys picks the token.  The result is bit-identical
+ * to the unsharded call.  The (global) vocabulary is at most 2^18 tokens (B200_EUNSUPPORTED above that).
+ * B200_EINVAL: NULL logits / temperatures / workspace (or both out and out_keys), rows or vocab <= 0, stage outside
+ * 0..3, logits not 16-byte aligned or a row stride not a multiple of 8. */
+int64_t b200_sample_filter_workspace_words(int rows);
+int b200_sample_filter_stage(const void* logits, int64_t logits_stride0, const float* temperatures, const int32_t* top_k,
+                             const float* top_p, const float* min_p, int rows, int vocab, int stage, int64_t* workspace,
+                             void* stream);
+int b200_sample_filtered(const void* logits, int64_t logits_stride0, const float* temperatures, const int32_t* top_k,
+                         const float* top_p, const float* min_p, int rows, int vocab, int64_t index_offset, uint64_t seed,
+                         uint64_t step, const int64_t* step_dev, int64_t* workspace, int64_t* out, int64_t* out_keys,
+                         void* stream);
+
 /* ---- decode-size projections on the tensor cores (wgmma; tests/test_gpu_linear.py) ---------------------------------
  *
  * F.linear of the reference's *ParallelLinear layers (layers/linear.py:51,73,153) for small batches, on wgmma,

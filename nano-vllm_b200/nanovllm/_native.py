@@ -40,6 +40,9 @@ SIGNATURES = {
     "b200_embedding": (_i, [_vp, _vp, _vp, _i, _i, _i64, _vp]),
     "b200_gather_tokens": (_i, [_vp, _vp, _vp, _i, _vp]),
     "b200_sample": (_i, [_vp, _i, _i64, _vp, _i, _i, _i64, _u64, _u64, _vp, _vp, _vp, _vp]),
+    "b200_sample_filter_workspace_words": (_i64, [_i]),
+    "b200_sample_filter_stage": (_i, [_vp, _i64, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
+    "b200_sample_filtered": (_i, [_vp, _i64, _vp, _vp, _vp, _vp, _i, _i, _i64, _u64, _u64, _vp, _vp, _vp, _vp, _vp]),
     # decode-size projections on wgmma (csrc/linear_tc.cu) and the fused LM head / layer tail experiments
     "b200_linear": (_i, [_vp, _i64, _vp, _vp, _i64, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "b200_add_rmsnorm_partials": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _f, _i, _vp]),

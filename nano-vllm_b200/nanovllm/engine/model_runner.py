@@ -165,6 +165,7 @@ class ModelRunner:
 
     def exit(self):
         self.graphs.clear()
+        self.fgraphs.clear()
         self.graph_pool = None
         torch.cuda.synchronize()
         if self._own_pg and dist.is_initialized():
@@ -188,6 +189,7 @@ class ModelRunner:
         prefill_bytes = _align(8) + 2 * _align(T * 8) + _align(T * 4) + 2 * _align((S + 1) * 4) + _align(S * 4) + _align(S * W * 4)
         if self.kv_fp8:                                      # the rebased cu_seqlens_q/k of at most S gather groups
             prefill_bytes += 2 * (8 * S + _ALIGN * S)
+        prefill_bytes += 3 * _align(S * 4)                   # top_k / top_p / min_p of a step where some request filters
         self.stage = _Staging(self.d_bytes, hosts=2)         # ping-pong: step N+1 is staged while step N runs
         self.pstage = _Staging(prefill_bytes)
         st = self.stage
@@ -215,6 +217,27 @@ class ModelRunner:
         self._done = [torch.cuda.Event(), torch.cuda.Event()]
         self._launches = 0
         self._pending: deque = deque()            # (read-back buffer, rows) of steps launched but not collected
+        # top-k / top-p / min-p: per-row parameters in their own small ping-pong staging (same index as the decode staging,
+        # uploaded only on a step where some row filters) and the filtered sampler's workspace, sized for cap_bs rows
+        self.f_off = {}
+        o = 0
+        for name in ("topk", "topp", "minp"):
+            self.f_off[name] = o
+            o = _align(o + mb * 4)
+        self.f_bytes = o
+        self.fstage = _Staging(self.f_bytes, hosts=2)
+        fspec = (("topk", np.int32, torch.int32), ("topp", np.float32, torch.float32), ("minp", np.float32, torch.float32))
+        self.hf = [{name: self.fstage.host_view(self.f_off[name], mb, npdt, k) for name, npdt, _ in fspec} for k in range(2)]
+        self.f_any = [False, False]
+        gf = {name: self.fstage.dev_view(self.f_off[name], mb, npdt, tdt) for name, npdt, tdt in fspec}
+        self.g_topk, self.g_topp, self.g_minp = gf["topk"], gf["topp"], gf["minp"]
+        self.g_topk.zero_()
+        self.g_topp.fill_(1.0)
+        self.g_minp.zero_()
+        self.g_filter_ws = ops.filter_workspace(self.cap_bs)
+        self.step_filters = None                  # the filter tensors of the step being launched (None: plain sampler)
+        self.fgraphs: dict[int, torch.cuda.CUDAGraph] = {}
+        self.fgraph_kernels: dict[int, int] = {}
 
     # ---- init-time passes -----------------------------------------------------------------------
     def warmup_model(self):
@@ -327,8 +350,24 @@ class ModelRunner:
         return dict(input_ids=ids, positions=lens - 1, slot_mapping=slots.astype(np.int32),
                     context_lens=lens.astype(np.int32), block_tables=self.prepare_block_tables(seqs))
 
+    def filter_arrays(self, seqs: list[Sequence], padded: int | None = None):
+        """Per-row top_k (int32), top_p and min_p (fp32) of a step over `padded` rows, or None when no row filters.
+        Greedy rows and graph-padding rows carry "off" (0, 1.0, 0.0)."""
+        if not any(s.temperature > 0 and (s.top_k > 0 or s.top_p < 1.0 or s.min_p > 0.0) for s in seqs):
+            return None
+        n = len(seqs)
+        padded = n if padded is None else padded
+        k = np.zeros(padded, np.int32)
+        p = np.ones(padded, np.float32)
+        mp = np.zeros(padded, np.float32)
+        for i, s in enumerate(seqs):
+            if s.temperature > 0:
+                k[i], p[i], mp[i] = max(s.top_k, 0), s.top_p, s.min_p
+        return k, p, mp
+
     def prepare_prefill(self, seqs: list[Sequence]):
         a = self.prefill_arrays(seqs)
+        filt = self.filter_arrays(seqs)
         st = self.pstage
         off = 0
         views = {}
@@ -345,6 +384,8 @@ class ModelRunner:
                                          plan_kv_groups(a["cu_seqlens_k"], self.kv_scratch_rows))
                 for i, g in enumerate(groups):
                     plan += [(f"g{i}q", g[6], torch.int32), (f"g{i}k", g[7], torch.int32)]
+        if filt is not None:
+            plan += [("topk", filt[0], torch.int32), ("topp", filt[1], torch.float32), ("minp", filt[2], torch.float32)]
         for name, arr, tdt in plan:
             h, d = st.views(off, arr.size, arr.dtype, tdt)
             h[:] = arr
@@ -361,6 +402,7 @@ class ModelRunner:
             kv_groups = [KVGroup(*g[:6], views[f"g{i}q"], views[f"g{i}k"]) for i, g in enumerate(groups)]
         set_context(True, views["cu_seqlens_q"], views["cu_seqlens_k"], a["max_seqlen_q"], a["max_seqlen_k"],
                     slot, None, bt, kv_groups)
+        self.step_filters = None if filt is None else (views["topk"], views["topp"], views["minp"])
         return views["input_ids"], views["positions"], views["temps"], views["step"]
 
     def _padded_rows(self, n: int) -> int:
@@ -390,6 +432,11 @@ class ModelRunner:
             h["temp"][n:padded] = 0
         bt = a["block_tables"]
         h["bt"][:n, :bt.shape[1]] = bt
+        filt = self.filter_arrays(seqs, padded)
+        self.f_any[k] = filt is not None
+        if filt is not None:
+            hf = self.hf[k]
+            hf["topk"][:padded], hf["topp"][:padded], hf["minp"][:padded] = filt
         return k
 
     def prepare_decode(self, seqs: list[Sequence], padded: int, staged: int | None = None, src=None):
@@ -410,15 +457,25 @@ class ModelRunner:
         nbytes = self.d_off["bt"] + padded * self.max_blocks * 4
         self.stage.upload(nbytes, k)
         self.h2d_bytes_last = nbytes
+        self.step_filters = None
+        if self.f_any[k]:                                    # only a step where some row filters uploads its parameters
+            self.fstage.upload(self.f_bytes, k)
+            self.h2d_bytes_last += self.f_bytes
+            self.step_filters = (self.g_topk[:padded], self.g_topp[:padded], self.g_minp[:padded])
         if src is not None:
             ops.gather_tokens(self.g_ids[:n], self.g_src[:n], self.g_tokens)
         set_context(False, slot_mapping=self.g_slot[:padded], context_lens=self.g_ctx[:padded],
                     block_tables=self.g_bt[:padded])
 
     # ---- model + sampling -------------------------------------------------------------------------
-    def _forward_and_sample(self, input_ids, positions, temps, step_dev, rows: int):
-        """hidden -> shard logits -> sampled token ids in self.g_tokens[:rows] (all enqueued, no sync)."""
+    def _forward_and_sample(self, input_ids, positions, temps, step_dev, rows: int, filters=None):
+        """hidden -> shard logits -> sampled token ids in self.g_tokens[:rows] (all enqueued, no sync).
+        ``filters``: (top_k, top_p, min_p) device tensors of the rows when some row filters; the logits are then
+        materialised (also under B200_LM_HEAD=fused) and sampled by the filtered sampler."""
         hidden = self.model(input_ids, positions)
+        if filters is not None:
+            self._sample_filtered(hidden, temps, step_dev, rows, filters)
+            return
         if self.fused_lm_head and rows <= self.g_keyws.numel():
             # opt-in (B200_LM_HEAD=fused): LM head + sampling in one tensor-core kernel, logits never written; parity-green but
             # slower than the library GEMM + sample_kernel pair (DESIGN.md 3.4), hence not the default
@@ -443,6 +500,27 @@ class ModelRunner:
             dist.all_reduce(keys, op=dist.ReduceOp.MAX)
             self.g_tokens[:rows].copy_(ops.tokens_from_keys(keys))
 
+    def _sample_filtered(self, hidden, temps, step_dev, rows: int, filters):
+        top_k, top_p, min_p = filters
+        logits = self.model.compute_logits(hidden)
+        if self.world_size == 1:
+            ops.sample_filtered(logits, temps, top_k, top_p, min_p, self.sample_seed, 0, self.g_filter_ws,
+                                out=self.g_tokens[:rows], step_dev=step_dev)
+            return
+        # every rank launches every stage and every all-reduce, whatever its rows need, so the collectives match
+        keys = self.g_keys[:rows]
+        ops.sample_filtered(logits, temps, top_k, top_p, min_p, self.sample_seed, 0, self.g_filter_ws, out=self.g_tokens[:rows],
+                            index_offset=self.vocab_offset, out_keys=keys, step_dev=step_dev, reduce=self._reduce_filter_words)
+        dist.all_reduce(keys, op=dist.ReduceOp.MAX)
+        self.g_tokens[:rows].copy_(ops.tokens_from_keys(keys))
+
+    @staticmethod
+    def _reduce_filter_words(words: torch.Tensor, op: str) -> None:
+        """All-reduce one stage's words of the filter workspace over the tensor-parallel ranks (a strided view)."""
+        buf = words.contiguous()
+        dist.all_reduce(buf, op=dist.ReduceOp.MAX if op == "max" else dist.ReduceOp.SUM)
+        words.copy_(buf)
+
     def run(self, seqs: list[Sequence], is_prefill: bool) -> list[int]:
         self.launch(seqs, is_prefill)
         return self.collect()
@@ -460,7 +538,7 @@ class ModelRunner:
             if prof is not None:
                 ev0 = torch.cuda.Event(enable_timing=True)
                 ev0.record()
-            self._forward_and_sample(ids, pos, temps, step_dev, n)
+            self._forward_and_sample(ids, pos, temps, step_dev, n, filters=self.step_filters)
         else:
             if n > self.cap_bs:
                 raise RuntimeError(f"decode batch {n} exceeds max_num_seqs = {self.cap_bs}")
@@ -469,11 +547,18 @@ class ModelRunner:
             if prof is not None:
                 ev0 = torch.cuda.Event(enable_timing=True)
                 ev0.record()
+            filt = self.step_filters
             if padded in self.graphs and not self.enforce_eager and n <= self.max_bs:
-                self.graphs[padded].replay()
-                ops.LAUNCHES[0] += self.graph_kernels[padded]
+                if filt is None:
+                    self.graphs[padded].replay()
+                    ops.LAUNCHES[0] += self.graph_kernels[padded]
+                else:                                        # the bucket's second graph: same step, filtered sampler
+                    self.fgraphs[padded].replay()
+                    ops.LAUNCHES[0] += self.fgraph_kernels[padded]
             else:
-                self._forward_and_sample(self.g_ids[:n], self.g_pos[:n], self.g_temp[:n], self.g_step, n)
+                if filt is not None:
+                    filt = tuple(t[:n] for t in filt)
+                self._forward_and_sample(self.g_ids[:n], self.g_pos[:n], self.g_temp[:n], self.g_step, n, filters=filt)
         if prof is not None:
             ev1 = torch.cuda.Event(enable_timing=True)
             ev1.record()
@@ -538,5 +623,20 @@ class ModelRunner:
             if self.graph_pool is None:
                 self.graph_pool = graph.pool()
             self.graphs[bs] = graph
+            torch.cuda.synchronize()
+            reset_context()
+        # second set, same pool: the same steps with the top-k / top-p / min-p sampler, replayed when some row filters
+        for bs in reversed(self.graph_bs):
+            set_context(False, slot_mapping=self.g_slot[:bs], context_lens=self.g_ctx[:bs], block_tables=self.g_bt[:bs])
+            args = (self.g_ids[:bs], self.g_pos[:bs], self.g_temp[:bs], self.g_step, bs)
+            filters = (self.g_topk[:bs], self.g_topp[:bs], self.g_minp[:bs])
+            self._forward_and_sample(*args, filters=filters)
+            torch.cuda.synchronize()
+            graph = torch.cuda.CUDAGraph()
+            before = ops.LAUNCHES[0]
+            with torch.cuda.graph(graph, self.graph_pool):
+                self._forward_and_sample(*args, filters=filters)
+            self.fgraph_kernels[bs] = ops.LAUNCHES[0] - before
+            self.fgraphs[bs] = graph
             torch.cuda.synchronize()
             reset_context()

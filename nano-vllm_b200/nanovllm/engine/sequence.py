@@ -27,7 +27,7 @@ class Sequence:
 
     __slots__ = ("seq_id", "status", "token_ids", "last_token", "num_tokens", "num_prompt_tokens",
                  "num_cached_tokens", "num_scheduled_tokens", "is_prefill", "block_table",
-                 "temperature", "max_tokens", "ignore_eos")
+                 "temperature", "max_tokens", "ignore_eos", "top_k", "top_p", "min_p")
 
     def __init__(self, token_ids: list[int], sampling_params: SamplingParams = _DEFAULT_SP):
         if not token_ids:
@@ -44,6 +44,9 @@ class Sequence:
         self.temperature = sampling_params.temperature
         self.max_tokens = sampling_params.max_tokens
         self.ignore_eos = sampling_params.ignore_eos
+        self.top_k = sampling_params.top_k
+        self.top_p = sampling_params.top_p
+        self.min_p = sampling_params.min_p
 
     def __len__(self) -> int:
         return self.num_tokens

@@ -276,6 +276,79 @@ def sample(logits: torch.Tensor, temperatures: torch.Tensor | None, seed: int, s
     return out
 
 
+FILTER_ROW_WORDS = 1538                    # int64 words per row of the filter workspace (include/b200_paged_attn.h)
+_FILTER_STAGE_WORDS = ((0, 1), (2, 514), (514, 1026), (1026, 1538))    # [lo, hi) of each stage's words within a row
+FILTER_TAU_WORD = 1
+
+
+def filter_workspace(rows: int, device="cuda") -> torch.Tensor:
+    """Zeroed workspace of ``sample_filtered`` for up to ``rows`` rows (every call leaves it zero again)."""
+    n = nat.load().b200_sample_filter_workspace_words(rows)
+    if n <= 0:
+        raise nat.B200Error("bad filter workspace row count")
+    return torch.zeros(n, dtype=torch.int64, device=device)
+
+
+def filter_stage_words(workspace: torch.Tensor, rows: int, stage: int) -> torch.Tensor:
+    """The words stage ``stage`` writes for ``rows`` rows, a [rows, n] strided view (all-reduce MAX for stage 0, SUM
+    for stages 1-3 under vocab parallelism)."""
+    lo, hi = _FILTER_STAGE_WORDS[stage]
+    return workspace[:rows * FILTER_ROW_WORDS].view(rows, FILTER_ROW_WORDS)[:, lo:hi]
+
+
+def filter_tau_keys(workspace: torch.Tensor, rows: int) -> torch.Tensor:
+    """Per row, the order-preserving 16-bit key of the threshold tau of the last ``sample_filtered`` call (0 = no filter)."""
+    return workspace[:rows * FILTER_ROW_WORDS].view(rows, FILTER_ROW_WORDS)[:, FILTER_TAU_WORD]
+
+
+def sample_filtered(logits: torch.Tensor, temps: torch.Tensor, top_k: torch.Tensor | None, top_p: torch.Tensor | None,
+                    min_p: torch.Tensor | None, seed: int, step: int, workspace: torch.Tensor, out: torch.Tensor | None = None,
+                    index_offset: int = 0, out_keys: torch.Tensor | None = None, step_dev: torch.Tensor | None = None,
+                    reduce=None) -> torch.Tensor:
+    """Top-k / top-p / min-p sampling: bf16 logits [rows, vocab] -> int64 token ids, as ``sample`` restricted per row to
+    {x >= tau} (include/b200_paged_attn.h).  ``top_k`` int32 [rows] (<= 0 off), ``top_p`` / ``min_p`` fp32 [rows]
+    (>= 1 / <= 0 off), each may be None; ``workspace`` from ``filter_workspace``.  Runs stages 0-3 and the race; after
+    stage s it calls ``reduce(filter_stage_words(workspace, rows, s), "max" if s == 0 else "sum")`` when ``reduce`` is
+    given (the vocab-parallel all-reduce of the stage's words)."""
+    assert logits.dim() == 2 and logits.stride(1) == 1 and logits.is_cuda
+    if logits.dtype == torch.float32:
+        nat.check(-2)                               # B200_EUNSUPPORTED: the filtered sampler reads bf16 logits only
+    _need(logits, torch.bfloat16, "logits"); _need(temps, torch.float32, "temps"); _need(workspace, torch.int64, "workspace")
+    if top_k is not None:
+        _need(top_k, torch.int32, "top_k")
+    for t, name in ((top_p, "top_p"), (min_p, "min_p")):
+        if t is not None:
+            _need(t, torch.float32, name)
+    rows, vocab = logits.shape
+    assert workspace.numel() >= rows * FILTER_ROW_WORDS, "filter workspace too small"
+    if out is None and out_keys is None:
+        out = torch.empty(rows, dtype=torch.int64, device=logits.device)
+    for stage in range(4):
+        sample_filter_stage(stage, logits, temps, top_k, top_p, min_p, workspace)
+        if reduce is not None:
+            reduce(filter_stage_words(workspace, rows, stage), "max" if stage == 0 else "sum")
+    sample_filter_race(logits, temps, top_k, top_p, min_p, seed, step, workspace, out, index_offset, out_keys, step_dev)
+    return out if out is not None else out_keys
+
+
+def sample_filter_race(logits, temps, top_k, top_p, min_p, seed: int, step: int, workspace: torch.Tensor, out=None,
+                       index_offset: int = 0, out_keys=None, step_dev=None) -> None:
+    """The last launch of ``sample_filtered``: the exponential race over {x >= tau} (workspace reduced by then)."""
+    rows, vocab = logits.shape
+    nat.check(nat.load().b200_sample_filtered(logits.data_ptr(), logits.stride(0), temps.data_ptr(), _ptr(top_k), _ptr(top_p),
+                                              _ptr(min_p), rows, vocab, index_offset, seed & (2**64 - 1), step & (2**64 - 1),
+                                              _ptr(step_dev), workspace.data_ptr(), _ptr(out), _ptr(out_keys), _stream()))
+
+
+def sample_filter_stage(stage: int, logits: torch.Tensor, temps: torch.Tensor, top_k, top_p, min_p,
+                        workspace: torch.Tensor) -> None:
+    """One threshold stage (0-3) of ``sample_filtered`` (for callers that reduce the stages' words themselves)."""
+    rows, vocab = logits.shape
+    nat.check(nat.load().b200_sample_filter_stage(logits.data_ptr(), logits.stride(0), temps.data_ptr(), _ptr(top_k),
+                                                  _ptr(top_p), _ptr(min_p), rows, vocab, stage, workspace.data_ptr(),
+                                                  _stream()))
+
+
 def tokens_from_keys(keys: torch.Tensor) -> torch.Tensor:
     """Decode the token ids out of (all-reduced) sample keys."""
     return 0xffffffff - (keys & 0xffffffff)
