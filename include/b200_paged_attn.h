@@ -192,8 +192,11 @@ int b200_qknorm_rope_store(b200_ctx* ctx, int layer, void* qkv, int64_t qkv_stri
  * flag_offset of every slice (zeroed once); epoch / done are two private zero-initialised device words; *err_flag
  * (device int, may be NULL) is set to 1 if a peer did not announce itself within ~18 s (the launch then completes with
  * undefined output instead of spinning forever).  Computes, on every rank, bit-identically:
- *   residual <- bf16(residual + sum_p partial_p);  out = norm(that fp32 sum) * weight.
- * Callers alternate two data offsets between consecutive calls (see csrc/tp_allreduce.cu for the protocol). */
+ *   s = (((residual + partial_0) + partial_1) + ... + partial_{world-1}),  every addition in fp32, in that order;
+ *   residual <- bf16(s), the one rounding;  out = bf16(s * rsqrt(mean(s^2) + eps) * weight).
+ * The residual comes first and the partials follow in rank order whichever rank computes: that fixed order is what
+ * makes the ranks agree bit for bit.  Callers alternate two data offsets between consecutive calls (see
+ * csrc/tp_allreduce.cu for the protocol). */
 int b200_allreduce_add_rmsnorm(const void* peer_bases_dev, uint64_t data_offset, uint64_t flag_offset,
                                int* epoch, unsigned int* done, int* err_flag, int rank, int world,
                                void* residual, const void* weight, void* out, int rows, int cols, float eps,

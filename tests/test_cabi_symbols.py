@@ -156,6 +156,12 @@ def test_argument_validation_needs_no_gpu():
     assert lib.b200_allreduce_add_rmsnorm(p, 0, 0, p, p, p, 2, 2, p, p, p, 1, 1024, 1e-6, None) == EINVAL
     assert lib.b200_allreduce_add_rmsnorm(p, 0, 0, p, p, p, 0, 2, p, p, p, 1, 1001, 1e-6, None) == EUNSUPPORTED
     assert lib.b200_allreduce_add_rmsnorm(p, 0, 0, p, p, p, 0, 2, p, p, p, 0, 1024, 1e-6, None) == 0
+    assert lib.b200_allreduce_add_rmsnorm(p, 0, 0, p, p, p, 0, 2, p, p, p, 1, 8200, 1e-6, None) == EUNSUPPORTED
+    assert lib.b200_allreduce_add_rmsnorm(p, 8, 0, p, p, p, 0, 2, p, p, p, 1, 1024, 1e-6, None) == EUNSUPPORTED  # data 16 B
+    assert lib.b200_allreduce_add_rmsnorm(p, 0, 2, p, p, p, 0, 2, p, p, p, 1, 1024, 1e-6, None) == EUNSUPPORTED  # flags 4 B
+    assert lib.b200_allreduce_add_rmsnorm(p, 0, 0, p, p, p, -1, 2, p, p, p, 1, 1024, 1e-6, None) == EINVAL
+    assert lib.b200_allreduce_add_rmsnorm(p, 0, 0, None, p, p, 0, 2, p, p, p, 1, 1024, 1e-6, None) == EINVAL   # no epoch
+    assert lib.b200_allreduce_add_rmsnorm(p, 0, 0, p, None, p, 0, 2, p, p, p, 1, 1024, 1e-6, None) == EINVAL   # no done
     assert lib.b200_allreduce_add_rmsnorm_nvls(p, None, 0, 0, p, p, p, 0, 2, p, p, p, 1, 1024, 1e-6, None) == EINVAL
     assert lib.b200_allreduce_add_rmsnorm_nvls(p, p, 0, 0, p, p, p, 0, 9, p, p, p, 1, 1024, 1e-6, None) == EINVAL
     assert lib.b200_allreduce_add_rmsnorm_nvls(p, p, 0, 0, p, p, p, 0, 2, p, p, p, 0, 1024, 1e-6, None) == 0

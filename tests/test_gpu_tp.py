@@ -33,8 +33,8 @@ def test_tp2_spawned_by_the_engine():
 def test_tp2_on_one_gpu_over_gloo():
     """Runs on EVERY GPU box, including single-GPU ones: two tensor-parallel ranks time-slice GPU 0 and reduce through
     gloo (eager).  Covers the head / MLP-column / vocabulary sharding, the (score, token) key combine and the SPMD
-    engine replicas end to end against the oracle; the NVLink exchange kernel itself needs two GPUs (tests above and the
-    parity leg of bench.py at N > 1)."""
+    engine replicas end to end against the oracle.  The exchange kernel over real NVLink needs two GPUs (tests above and
+    the parity leg of bench.py at N > 1); its data path and flag protocol run on one GPU in test_gpu_tp_exchange.py."""
     env = dict(os.environ, TP_EAGER="1", B200_TP_BACKEND="gloo", B200_TP_ONE_DEVICE="1", B200_TP_ALLREDUCE="nccl")
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
            "--master-port", "29557", os.path.join(ROOT, "tests", "tp_worker.py")]
