@@ -307,6 +307,51 @@ int b200_penalty_apply(void* logits, int64_t logits_stride0, int rows, int vocab
                        int32_t* lengths, int num_slots, int capacity, const int32_t* slots, const int64_t* pending,
                        const float* repetition, const float* frequency, const float* presence, void* stream);
 
+/* Per-token logprobs of the raw logits (vLLM v1's raw_logprobs; the reference has none).  bf16 logits only.
+ * Per row r with k[r] >= 0 (k[r] = -1: off, every call returns at once for the row; k above 20 is taken as 20), over the
+ * logits as the LM head wrote them (before penalties, temperature and filters):
+ *   logprob(x) = (x - m) - ln(S * 2^-40), m = the row maximum, S = sum_j round(exp(x_j - m) * 2^40) (uint64, expf),
+ *   computed in float64 and rounded once to fp32;
+ *   rank = #{j : x_j >= x_t} for the sampled token t (at least 1; ties raise it);
+ *   the top k: the k largest x_j, value descending then token id ascending.
+ * Call order: b200_logprob_topk and (for penalised rows) b200_logprob_save before b200_penalty_apply; after the token is
+ * known, b200_logprob_restore, b200_logprob_rank, b200_logprob_finish.  All on the same rows, k, logits and workspace.
+ *
+ * workspace: b200_logprob_workspace_words(rows) int64 words (0 for rows <= 0 or > 1024), zero before the first use; the
+ * finish leaves every word of a logprob row zero again.  Row r owns words [r * 8, r * 8 + 8):
+ *   word 0   written by b200_logprob_topk, reduce with MAX: order-preserving key of m (as word 1 of the filter workspace)
+ *   word 1   written by b200_logprob_restore, reduce with MAX: key of x_t (0 on a shard that does not hold t)
+ *   word 2   written by b200_logprob_rank, reduce with SUM: S
+ *   word 3   written by b200_logprob_rank, reduce with SUM: the rank
+ *   word 4   number of saved pairs (b200_logprob_save -> b200_logprob_restore), local to the rank
+ * topk_keys: int64 [rows, 20]; row r's first max(k[r], 1) words are its shard's largest logits as b200_sample keys
+ *   (value << 32 | 0xffffffff - global id, order-preserving, -0 as +0), not accumulated: nothing to zero.
+ * saved: int64 [rows, capacity + 1], the raw bf16 of every logit b200_penalty_apply will rewrite for the row (its slot's
+ *   entries and the pending token, read as the apply reads them), as column << 16 | bits, -1 = none.
+ * b200_logprob_restore writes them back (saved may be NULL when no row was penalised) and reads x_t from tokens[r].
+ * b200_logprob_finish merges `sources` top-k lists, topk_keys being [sources, rows, 20], and writes per row:
+ *   out_ids[r * out_stride + 0] = t, out_logprobs[... + 0] = logprob(x_t), out_rank[r * out_stride] = rank,
+ *   out_ids / out_logprobs[r * out_stride + 1 + i], i < k[r]: the i-th largest token and its logprob.
+ * Vocab-parallel use: each rank passes its shard with index_offset = its first vocab id, all-reduces word 0 (MAX) after
+ * b200_logprob_topk, word 1 (MAX) after b200_logprob_restore, words 2-3 (SUM) after b200_logprob_rank, gathers topk_keys
+ * over the ranks and passes sources = world.  The result is bit-identical to the unsharded call.
+ * B200_EINVAL: a NULL pointer (other than pending and restore's saved), rows <= 0 or > 1024, vocab <= 0, index_offset
+ *   < 0, logits not 16-byte aligned, a row stride not a multiple of 8 or < vocab with rows > 1, num_slots / capacity <= 0
+ *   (save), sources outside 1..64 or out_stride < 21 (finish).  B200_EUNSUPPORTED: a global vocabulary above 2^18. */
+int64_t b200_logprob_workspace_words(int rows);
+int b200_logprob_topk(const void* logits, int64_t logits_stride0, const int32_t* k, int rows, int vocab, int64_t index_offset,
+                      int64_t* workspace, int64_t* topk_keys, void* stream);
+int b200_logprob_save(const void* logits, int64_t logits_stride0, const int32_t* k, int rows, int vocab, int64_t index_offset,
+                      const int64_t* history, const int32_t* lengths, int num_slots, int capacity, const int32_t* slots,
+                      const int64_t* pending, int64_t* workspace, int64_t* saved, void* stream);
+int b200_logprob_restore(void* logits, int64_t logits_stride0, const int32_t* k, int rows, int vocab, int64_t index_offset,
+                         const int64_t* tokens, int64_t* workspace, const int64_t* saved, int capacity, void* stream);
+int b200_logprob_rank(const void* logits, int64_t logits_stride0, const int32_t* k, int rows, int vocab, int64_t* workspace,
+                      void* stream);
+int b200_logprob_finish(const int32_t* k, int rows, const int64_t* tokens, const int64_t* topk_keys, int sources,
+                        int64_t* workspace, int32_t* out_ids, float* out_logprobs, int32_t* out_rank, int64_t out_stride,
+                        void* stream);
+
 /* ---- decode-size projections on the tensor cores (wgmma; tests/test_gpu_linear.py) ---------------------------------
  *
  * F.linear of the reference's *ParallelLinear layers (layers/linear.py:51,73,153) for small batches, on wgmma,

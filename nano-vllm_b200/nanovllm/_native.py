@@ -45,6 +45,12 @@ SIGNATURES = {
     "b200_sample_filtered": (_i, [_vp, _i64, _vp, _vp, _vp, _vp, _i, _i, _i64, _u64, _u64, _vp, _vp, _vp, _vp, _vp]),
     "b200_penalty_load": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _i, _vp]),
     "b200_penalty_apply": (_i, [_vp, _i64, _i, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b200_logprob_workspace_words": (_i64, [_i]),
+    "b200_logprob_topk": (_i, [_vp, _i64, _vp, _i, _i, _i64, _vp, _vp, _vp]),
+    "b200_logprob_save": (_i, [_vp, _i64, _vp, _i, _i, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "b200_logprob_restore": (_i, [_vp, _i64, _vp, _i, _i, _i64, _vp, _vp, _vp, _i, _vp]),
+    "b200_logprob_rank": (_i, [_vp, _i64, _vp, _i, _i, _vp, _vp]),
+    "b200_logprob_finish": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i64, _vp]),
     # decode-size projections on wgmma (csrc/linear_tc.cu) and the fused LM head / layer tail experiments
     "b200_linear": (_i, [_vp, _i64, _vp, _vp, _i64, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "b200_add_rmsnorm_partials": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _f, _i, _vp]),

@@ -19,7 +19,8 @@ from dataclasses import fields
 from time import perf_counter
 
 from ..config import Config
-from ..sampling_params import SamplingParams
+from ..ops import LOGPROB_LP_COL, LOGPROB_RANK_COL
+from ..sampling_params import Logprob, SamplingParams
 from .model_runner import ModelRunner
 from .scheduler import Scheduler
 from .sequence import Sequence
@@ -30,6 +31,24 @@ def _free_port() -> int:
     with socket.socket() as s:
         s.bind(("127.0.0.1", 0))
         return s.getsockname()[1]
+
+
+def logprob_dicts(rows: list, k: int) -> tuple[list[dict], float]:
+    """A finished sequence's logprob rows (one packed int32 row per completion token, ModelRunner.collect) -> one
+    {token_id: Logprob} dict per token and the cumulative logprob of the sampled tokens.  Built like vLLM's: the sampled
+    token first, with its rank, then the top k with ranks 1..k; a sampled token inside the top k takes its top-k entry."""
+    import numpy as np
+    a = np.stack(rows) if rows else np.zeros((0, LOGPROB_RANK_COL + 1), np.int32)
+    ids = a[:, :1 + k].tolist()
+    lps = a[:, LOGPROB_LP_COL:LOGPROB_LP_COL + 1 + k].view(np.float32).tolist()
+    ranks = a[:, LOGPROB_RANK_COL].tolist()
+    out = []
+    for tid, tlp, rank in zip(ids, lps, ranks):
+        d = {tid[0]: Logprob(tlp[0], rank)}
+        for j in range(1, k + 1):
+            d[tid[j]] = Logprob(tlp[j], j)
+        out.append(d)
+    return out, sum(t[0] for t in lps)
 
 
 def _worker_main(model: str, kwargs: dict, rank: int, world: int, port: int):
@@ -151,8 +170,14 @@ class LLMEngine:
     def _step(self):
         seqs, is_prefill = self.scheduler.schedule()
         num_tokens = sum(s.num_scheduled_tokens for s in seqs) if is_prefill else -len(seqs)
+        before = [s.num_tokens for s in seqs]
         token_ids = self.model_runner.call("run", seqs, is_prefill)
         self.scheduler.postprocess(seqs, token_ids, is_prefill)
+        lp = getattr(self.model_runner, "last_logprobs", None)
+        if lp is not None:
+            for i, (s, b) in enumerate(zip(seqs, before)):
+                if s.num_tokens != b and s.logprob_rows is not None:
+                    s.logprob_rows.append(lp[i].copy())   # not a view: it would keep the step's rows alive
         outputs = [(s.seq_id, s.completion_token_ids) for s in seqs if s.is_finished]
         return outputs, num_tokens
 
@@ -185,6 +210,9 @@ class LLMEngine:
             for seq in finished:                  # detokenise now: the next step is already running on the GPU
                 toks = seq.completion_token_ids
                 done[seq.seq_id] = {"text": self.tokenizer.decode(toks), "token_ids": toks}
+                if seq.logprob_rows is not None:
+                    lp, cum = logprob_dicts(seq.logprob_rows, seq.logprobs_k)
+                    done[seq.seq_id].update(logprobs=lp, cumulative_logprob=cum)
             if pbar is not None:
                 pbar.set_postfix({"Prefill": f"{int(stats['prefill'])}tok/s", "Decode": f"{int(stats['decode'])}tok/s"})
                 pbar.update(len(finished))
@@ -241,15 +269,24 @@ class LLMEngine:
                 tw = perf_counter()
                 tokens = runner.call("collect")
                 st["wait_s"] += perf_counter() - tw
-                for s, b, t in zip(seqs, before, tokens):
+                lp = getattr(runner, "last_logprobs", None)
+                for i, (s, b, t) in enumerate(zip(seqs, before, tokens)):
                     if s.num_tokens != b:                       # a token was appended: give it its value
                         s.token_ids[-1] = t
                         s.last_token = t
+                        if lp is not None and s.logprob_rows is not None:
+                            s.logprob_rows.append(lp[i].copy())
             else:
                 tw = perf_counter()
                 tokens = runner.call("collect")
                 st["wait_s"] += perf_counter() - tw
+                lp = getattr(runner, "last_logprobs", None)
+                before = None if lp is None else [s.num_tokens for s in seqs]
                 sched.postprocess(seqs, tokens, is_prefill)
+                if lp is not None:
+                    for i, (s, b) in enumerate(zip(seqs, before)):
+                        if s.num_tokens != b and s.logprob_rows is not None:
+                            s.logprob_rows.append(lp[i].copy())
                 if not sched.is_finished():
                     nxt = sched.schedule()
             now = perf_counter()

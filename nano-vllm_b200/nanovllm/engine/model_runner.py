@@ -22,6 +22,7 @@ from __future__ import annotations
 
 import os
 from collections import deque
+from time import perf_counter
 
 import numpy as np
 import torch
@@ -167,6 +168,7 @@ class ModelRunner:
     def exit(self):
         self.graphs.clear()
         self.fgraphs.clear()
+        self.lgraphs.clear()
         self.graph_pool = None
         torch.cuda.synchronize()
         if self._own_pg and dist.is_initialized():
@@ -187,13 +189,8 @@ class ModelRunner:
             self.d_off[name] = o
             o = _align(o + count * size)
         self.d_bytes = o
-        prefill_bytes = _align(8) + 2 * _align(T * 8) + _align(T * 4) + 2 * _align((S + 1) * 4) + _align(S * 4) + _align(S * W * 4)
-        if self.kv_fp8:                                      # the rebased cu_seqlens_q/k of at most S gather groups
-            prefill_bytes += 2 * (8 * S + _ALIGN * S)
-        prefill_bytes += 3 * _align(S * 4)                   # top_k / top_p / min_p of a step where some request filters
-        prefill_bytes += 4 * _align(S * 4) + _align((S + 1) * 4)   # penalty slot / r / f / p and entry-list offsets
         self.stage = _Staging(self.d_bytes, hosts=2)         # ping-pong: step N+1 is staged while step N runs
-        self.pstage = _Staging(prefill_bytes)
+        self.pstage = _Staging(self.prefill_staging_bytes(T, S, W, self.kv_fp8))
         st = self.stage
         spec = (("step", 1, np.int64, torch.int64), ("ids", mb, np.int64, torch.int64), ("pos", mb, np.int64, torch.int64),
                 ("slot", mb, np.int32, torch.int32), ("ctx", mb, np.int32, torch.int32), ("temp", mb, np.float32, torch.float32),
@@ -227,7 +224,7 @@ class ModelRunner:
                  ("minp", mb, np.float32, torch.float32), ("pslot", mb, np.int32, torch.int32),
                  ("prep", mb, np.float32, torch.float32), ("pfreq", mb, np.float32, torch.float32),
                  ("ppres", mb, np.float32, torch.float32), ("plslot", mb, np.int32, torch.int32),
-                 ("ploff", mb + 1, np.int32, torch.int32))
+                 ("ploff", mb + 1, np.int32, torch.int32), ("lpk", mb, np.int32, torch.int32))
         self.f_off = {}
         o = 0
         for name, cnt, _, _ in fspec:
@@ -239,12 +236,16 @@ class ModelRunner:
                    for k in range(2)]
         for h in self.hf:
             h["pslot"][:] = -1
+            h["lpk"][:] = -1
         self.f_any = [False, False]
+        self.lp_any = [False, False]              # whether the step staged in buffer k has a logprob row
         self.p_load: list = [None, None]          # (entries, rows) of a decode step that reloads slots, per staging buffer
         gf = {name: self.fstage.dev_view(self.f_off[name], cnt, npdt, tdt) for name, cnt, npdt, tdt in fspec}
         self.g_topk, self.g_topp, self.g_minp = gf["topk"], gf["topp"], gf["minp"]
         self.g_pslot, self.g_prep, self.g_pfreq, self.g_ppres = gf["pslot"], gf["prep"], gf["pfreq"], gf["ppres"]
         self.g_plslot, self.g_ploff = gf["plslot"], gf["ploff"]
+        self.g_lpk = gf["lpk"]
+        self.g_lpk.fill_(-1)
         self.g_topk.zero_()
         self.g_topp.fill_(1.0)
         self.g_minp.zero_()
@@ -258,6 +259,29 @@ class ModelRunner:
         self.fgraphs: dict[int, torch.cuda.CUDAGraph] = {}
         self.fgraph_kernels: dict[int, int] = {}
         self._init_penalty_slots(self.cap_bs)
+        # logprobs (DESIGN.md 3.3.2): the per-row k rides in the filter staging (-1 = off); workspace, top-k keys, the
+        # packed result rows and the saved raw logits live on the device (allocate_penalty_history, after the KV cache is
+        # sized), a pinned ping-pong copy of the result per read-back buffer, and a third graph set replayed only on a step
+        # with a logprob row
+        self.g_lp_ws = self.g_lp_keys = self.g_lp_out = self.g_lp_saved = None
+        self.h_lp = [torch.zeros(S, ops.LOGPROB_OUT_WORDS, dtype=torch.int32, pin_memory=True) for _ in range(2)]
+        self.h_lp_np = [t.numpy() for t in self.h_lp]
+        self.step_logprobs = None                 # the k tensor of the step being launched, or None
+        self.last_logprobs = None                 # packed result rows of the last collected step, or None
+        self.lgraphs: dict[int, torch.cuda.CUDAGraph] = {}
+        self.lgraph_kernels: dict[int, int] = {}
+
+    @staticmethod
+    def prefill_staging_bytes(T: int, S: int, W: int, kv_fp8: bool) -> int:
+        """Bytes of the prefill staging buffer: room for prepare_prefill's plan at its limits, T new tokens of S sequences
+        with block tables W wide, every optional region staged."""
+        n = _align(8) + 2 * _align(T * 8) + _align(T * 4) + 2 * _align((S + 1) * 4) + _align(S * 4) + _align(S * W * 4)
+        if kv_fp8:                                           # the rebased cu_seqlens_q/k of at most S gather groups
+            n += 2 * (8 * S + _ALIGN * S)
+        n += 3 * _align(S * 4)                               # top_k / top_p / min_p of a step where some request filters
+        n += 4 * _align(S * 4) + _align((S + 1) * 4)         # penalty slot / r / f / p and entry-list offsets
+        n += _align(S * 4)                                   # per-row logprobs k of a step where some request wants them
+        return n
 
     # ---- presence / frequency / repetition penalties (DESIGN.md 3.3.1) ------------------------------------------------
     def _init_penalty_slots(self, num_slots: int):
@@ -283,9 +307,16 @@ class ModelRunner:
         return config.max_num_seqs, min(config.max_model_len, config.hf_config.vocab_size)
 
     def allocate_penalty_history(self):
+        """The penalty history pool, and the logprob kernels' device buffers (their saved-logits buffer has a slot's
+        capacity plus one entry per row), all sized after the KV cache."""
         slots, capacity = self.penalty_pool_shape(self.config)
         self._init_penalty_slots(slots)
         self.pen_hist, self.pen_len = ops.penalty_history(slots, capacity)
+        S = self.cap_bs
+        self.g_lp_ws = ops.logprob_workspace(S)
+        self.g_lp_keys = torch.zeros(S * ops.LOGPROB_MAX_K, dtype=torch.int64, device="cuda")
+        self.g_lp_out = torch.zeros(S, ops.LOGPROB_OUT_WORDS, dtype=torch.int32, device="cuda")
+        self.g_lp_saved = ops.logprob_saved_buffer(S, capacity)
 
     @staticmethod
     def penalty_entries(seq: Sequence, num_tokens: int | None = None) -> np.ndarray:
@@ -507,9 +538,22 @@ class ModelRunner:
                 k[i], p[i], mp[i] = max(s.top_k, 0), s.top_p, s.min_p
         return k, p, mp
 
+    @staticmethod
+    def logprob_arrays(seqs: list[Sequence], padded: int | None = None, prefill: bool = False):
+        """Per-row requested logprobs k (int32, -1 = off) of a step over `padded` rows, or None when no row wants them.
+        In a prefill only the rows whose prompt ends in this step (the ones that sample) get theirs."""
+        if not any(s.logprobs_k >= 0 for s in seqs):
+            return None
+        n = len(seqs)
+        k = np.full(n if padded is None else padded, -1, np.int32)
+        k[:n] = [s.logprobs_k if not prefill or s.num_cached_tokens + s.num_scheduled_tokens >= s.num_tokens else -1
+                 for s in seqs]
+        return None if prefill and not (k >= 0).any() else k
+
     def prepare_prefill(self, seqs: list[Sequence]):
         a = self.prefill_arrays(seqs)
         filt = self.filter_arrays(seqs)
+        lpk = self.logprob_arrays(seqs, prefill=True)
         self.release_penalty_slots()
         pen = self.penalty_arrays(seqs, prefill=True)
         st = self.pstage
@@ -534,6 +578,8 @@ class ModelRunner:
             offsets, n_ent = self._stage_penalty_entries(seqs, pen[4], 2, prefill=True)
             plan += [("pslot", pen[0], torch.int32), ("prep", pen[1], torch.float32), ("pfreq", pen[2], torch.float32),
                      ("ppres", pen[3], torch.float32), ("poff", offsets, torch.int32)]
+        if lpk is not None:
+            plan.append(("lpk", lpk, torch.int32))
         for name, arr, tdt in plan:
             h, d = st.views(off, arr.size, arr.dtype, tdt)
             h[:] = arr
@@ -555,6 +601,7 @@ class ModelRunner:
         set_context(True, views["cu_seqlens_q"], views["cu_seqlens_k"], a["max_seqlen_q"], a["max_seqlen_k"],
                     slot, None, bt, kv_groups)
         self.step_filters = None if filt is None else (views["topk"], views["topp"], views["minp"])
+        self.step_logprobs = views.get("lpk")
         return views["input_ids"], views["positions"], views["temps"], views["step"]
 
     def _padded_rows(self, n: int) -> int:
@@ -587,7 +634,9 @@ class ModelRunner:
         filt = self.filter_arrays(seqs, padded)
         self.release_penalty_slots()
         pen = self.penalty_arrays(seqs, padded)
-        self.f_any[k] = filt is not None or pen is not None
+        lpk = self.logprob_arrays(seqs, padded)
+        self.f_any[k] = filt is not None or pen is not None or lpk is not None
+        self.lp_any[k] = lpk is not None
         self.p_load[k] = None
         if self.f_any[k]:
             hf = self.hf[k]
@@ -597,6 +646,7 @@ class ModelRunner:
             if pen is None:
                 pen = (-1, 1.0, 0.0, 0.0, np.zeros(padded, bool))
             hf["pslot"][:padded], hf["prep"][:padded], hf["pfreq"][:padded], hf["ppres"][:padded] = pen[:4]
+            hf["lpk"][:padded] = -1 if lpk is None else lpk
             load = pen[4][:n]
             if load.any():                                   # sequences whose slot was taken while outside the batch
                 offsets, total = self._stage_penalty_entries(seqs, load, k, prefill=False)
@@ -623,7 +673,7 @@ class ModelRunner:
         nbytes = self.d_off["bt"] + padded * self.max_blocks * 4
         self.stage.upload(nbytes, k)
         self.h2d_bytes_last = nbytes
-        self.step_filters = self.step_penalties = None
+        self.step_filters = self.step_penalties = self.step_logprobs = None
         if self.f_any[k]:                                    # only a step where some row filters or penalises uploads them
             self.fstage.upload(self.f_bytes, k)
             self.h2d_bytes_last += self.f_bytes
@@ -631,6 +681,8 @@ class ModelRunner:
             # the pending token of a row is its input id: the token sampled one step earlier, absorbed into the history
             self.step_penalties = (self.g_pslot[:padded], self.g_prep[:padded], self.g_pfreq[:padded], self.g_ppres[:padded],
                                    self.g_ids[:padded])
+            if self.lp_any[k]:
+                self.step_logprobs = self.g_lpk[:padded]
             if self.p_load[k] is not None:
                 total, rows = self.p_load[k]
                 self._load_penalty_slots(k, total, self.g_ploff[:rows + 1], self.g_plslot[:rows])
@@ -640,14 +692,16 @@ class ModelRunner:
                     block_tables=self.g_bt[:padded])
 
     # ---- model + sampling -------------------------------------------------------------------------
-    def _forward_and_sample(self, input_ids, positions, temps, step_dev, rows: int, filters=None, penalties=None):
+    def _forward_and_sample(self, input_ids, positions, temps, step_dev, rows: int, filters=None, penalties=None,
+                            logprobs=None):
         """hidden -> shard logits -> sampled token ids in self.g_tokens[:rows] (all enqueued, no sync).
         ``filters``: (top_k, top_p, min_p) device tensors of the rows when some row filters; ``penalties``: (slot,
         repetition, frequency, presence, pending token or None) when some row filters or penalises.  The logits are then
-        materialised (also under B200_LM_HEAD=fused), penalised and sampled by the filtered sampler."""
+        materialised (also under B200_LM_HEAD=fused), penalised and sampled by the filtered sampler.  ``logprobs``: the
+        rows' requested k (int32, -1 = off) when some row wants logprobs; they go into self.g_lp_out[:rows]."""
         hidden = self.model(input_ids, positions)
-        if filters is not None or penalties is not None:
-            self._sample_filtered(hidden, temps, step_dev, rows, filters, penalties)
+        if filters is not None or penalties is not None or logprobs is not None:
+            self._sample_filtered(hidden, temps, step_dev, rows, filters, penalties, logprobs)
             return
         if self.fused_lm_head and rows <= self.g_keyws.numel():
             # opt-in (B200_LM_HEAD=fused): LM head + sampling in one tensor-core kernel, logits never written; parity-green but
@@ -673,22 +727,41 @@ class ModelRunner:
             dist.all_reduce(keys, op=dist.ReduceOp.MAX)
             self.g_tokens[:rows].copy_(ops.tokens_from_keys(keys))
 
-    def _sample_filtered(self, hidden, temps, step_dev, rows: int, filters, penalties=None):
+    def _sample_filtered(self, hidden, temps, step_dev, rows: int, filters, penalties=None, logprobs=None):
         logits = self.model.compute_logits(hidden)
+        tp = self.world_size > 1
+        reduce = self._reduce_filter_words if tp else None
+        if logprobs is not None:                 # on the raw logits: top k and maximum, then keep what the penalties rewrite
+            ops.logprobs_topk(logits, logprobs, self.g_lp_ws, self.g_lp_keys, self.vocab_offset, reduce=reduce)
         if penalties is not None:                # every rank absorbs into its full copy of the history, penalises its shard
             slot, rep, freq, pres, pending = penalties
+            if logprobs is not None:
+                ops.logprobs_save(logits, logprobs, self.g_lp_ws, self.g_lp_saved, self.pen_hist, self.pen_len, slot, pending,
+                                  self.vocab_offset)
             ops.penalty_apply(logits, self.pen_hist, self.pen_len, slot, rep, freq, pres, pending, self.vocab_offset)
         top_k, top_p, min_p = filters if filters is not None else (None, None, None)
-        if self.world_size == 1:
+        if not tp:
             ops.sample_filtered(logits, temps, top_k, top_p, min_p, self.sample_seed, 0, self.g_filter_ws,
                                 out=self.g_tokens[:rows], step_dev=step_dev)
-            return
-        # every rank launches every stage and every all-reduce, whatever its rows need, so the collectives match
-        keys = self.g_keys[:rows]
-        ops.sample_filtered(logits, temps, top_k, top_p, min_p, self.sample_seed, 0, self.g_filter_ws, out=self.g_tokens[:rows],
-                            index_offset=self.vocab_offset, out_keys=keys, step_dev=step_dev, reduce=self._reduce_filter_words)
-        dist.all_reduce(keys, op=dist.ReduceOp.MAX)
-        self.g_tokens[:rows].copy_(ops.tokens_from_keys(keys))
+        else:
+            # every rank launches every stage and every all-reduce, whatever its rows need, so the collectives match
+            keys = self.g_keys[:rows]
+            ops.sample_filtered(logits, temps, top_k, top_p, min_p, self.sample_seed, 0, self.g_filter_ws,
+                                out=self.g_tokens[:rows], index_offset=self.vocab_offset, out_keys=keys, step_dev=step_dev,
+                                reduce=reduce)
+            dist.all_reduce(keys, op=dist.ReduceOp.MAX)
+            self.g_tokens[:rows].copy_(ops.tokens_from_keys(keys))
+        if logprobs is not None:                 # the logits are raw again after the restore
+            ops.logprobs_finish(logits, logprobs, self.g_tokens[:rows], self.g_lp_ws, self.g_lp_keys, self.g_lp_out,
+                                self.vocab_offset, saved=self.g_lp_saved if penalties is not None else None,
+                                capacity=self.pen_hist.shape[1] if penalties is not None else 0, reduce=reduce,
+                                gather=self._gather_logprob_keys if tp else None)
+
+    def _gather_logprob_keys(self, keys: torch.Tensor) -> torch.Tensor:
+        """Every tensor-parallel rank's top-k keys, [world, n] in rank order."""
+        out = torch.empty(self.world_size, keys.numel(), dtype=keys.dtype, device=keys.device)
+        dist.all_gather(list(out.unbind(0)), keys.contiguous())
+        return out
 
     @staticmethod
     def _reduce_filter_words(words: torch.Tensor, op: str) -> None:
@@ -714,7 +787,8 @@ class ModelRunner:
             if prof is not None:
                 ev0 = torch.cuda.Event(enable_timing=True)
                 ev0.record()
-            self._forward_and_sample(ids, pos, temps, step_dev, n, filters=self.step_filters, penalties=self.step_penalties)
+            self._forward_and_sample(ids, pos, temps, step_dev, n, filters=self.step_filters, penalties=self.step_penalties,
+                                     logprobs=self.step_logprobs)
         else:
             if n > self.cap_bs:
                 raise RuntimeError(f"decode batch {n} exceeds max_num_seqs = {self.cap_bs}")
@@ -723,9 +797,12 @@ class ModelRunner:
             if prof is not None:
                 ev0 = torch.cuda.Event(enable_timing=True)
                 ev0.record()
-            filt = self.step_filters
+            filt, lpk = self.step_filters, self.step_logprobs
             if padded in self.graphs and not self.enforce_eager and n <= self.max_bs:
-                if filt is None:
+                if lpk is not None:                          # the third graph: the second one plus the logprob kernels
+                    self.lgraphs[padded].replay()
+                    ops.LAUNCHES[0] += self.lgraph_kernels[padded]
+                elif filt is None:
                     self.graphs[padded].replay()
                     ops.LAUNCHES[0] += self.graph_kernels[padded]
                 else:                                        # the bucket's second graph: penalties, then the filtered sampler
@@ -736,14 +813,15 @@ class ModelRunner:
                 if filt is not None:
                     filt = tuple(t[:n] for t in filt)
                     pen = tuple(t[:n] for t in pen)
+                    lpk = None if lpk is None else lpk[:n]
                 self._forward_and_sample(self.g_ids[:n], self.g_pos[:n], self.g_temp[:n], self.g_step, n, filters=filt,
-                                         penalties=pen)
+                                         penalties=pen, logprobs=lpk)
         if prof is not None:
             ev1 = torch.cuda.Event(enable_timing=True)
             ev1.record()
             prof["events"].append((ev0, ev1))
             prof["h2d"] += self.h2d_bytes_last
-            prof["d2h"] += n * 8
+            prof["d2h"] += n * 8 + (n * ops.LOGPROB_OUT_WORDS * 4 if self.step_logprobs is not None else 0)
             prof["steps"] += 1
         kk = self._launches & 1
         self._launches += 1
@@ -752,19 +830,26 @@ class ModelRunner:
         peer = getattr(self.model, "peer", None)
         if peer is not None:              # the exchange kernel's timeout flag rides along with the tokens: checked every step
             self.h_err[kk].copy_(peer.state[2:3], non_blocking=True)
+        lp = self.step_logprobs is not None
+        if lp:                            # only a step with a logprob row reads its result rows back
+            self.h_lp[kk][:n].copy_(self.g_lp_out[:n], non_blocking=True)
         self._done[kk].record()
-        self._pending.append((kk, n))
-        self.d2h_bytes_last = n * 8
+        self._pending.append((kk, n, lp))
+        self.d2h_bytes_last = n * 8 + (n * ops.LOGPROB_OUT_WORDS * 4 if lp else 0)
+        self.step_logprobs = None
         reset_context()
 
     def collect(self) -> list[int]:
-        """Wait for the oldest step enqueued by launch() (that step's only host sync) and return its token ids."""
-        kk, n = self._pending.popleft()
+        """Wait for the oldest step enqueued by launch() (that step's only host sync) and return its token ids.  The step's
+        logprob result rows (int32 [n, ops.LOGPROB_OUT_WORDS], a copy) are left in self.last_logprobs, None when no row of
+        the step asked for logprobs; rows that did not are undefined."""
+        kk, n, lp = self._pending.popleft()
         self._done[kk].synchronize()
         if int(self.h_err[kk][0]) != 0:
             from .peer_reduce import PeerExchangeTimeout
             raise PeerExchangeTimeout("tensor-parallel peer exchange timed out in this step (a rank stopped or fell >10 s "
                                       "behind); its tokens are invalid -- rerun with B200_TP_ALLREDUCE=nccl to bypass")
+        self.last_logprobs = self.h_lp_np[kk][:n].copy() if lp else None
         return self.h_tokens_np[kk][:n].tolist()
 
     def drain(self) -> None:
@@ -789,6 +874,18 @@ class ModelRunner:
         h["step"][0] = 0
         self.stage.upload(self.d_bytes, 0)
         torch.cuda.synchronize()
+        # per graph set: cumulative capture seconds, bytes reserved by the caching allocator and bytes of the graphs' shared
+        # private pool after it
+        self.capture_stats: list[dict] = []
+        t0 = perf_counter()
+
+        def set_done(name: str):
+            pool = tuple(self.graph_pool)
+            pool_bytes = sum(seg["total_size"] for seg in torch.cuda.memory_snapshot()
+                             if tuple(seg.get("segment_pool_id", ())) == pool)
+            self.capture_stats.append(dict(set=name, seconds=perf_counter() - t0, reserved=torch.cuda.memory_reserved(),
+                                           pool=pool_bytes))
+
         for bs in reversed(self.graph_bs):
             set_context(False, slot_mapping=self.g_slot[:bs], context_lens=self.g_ctx[:bs], block_tables=self.g_bt[:bs])
             args = (self.g_ids[:bs], self.g_pos[:bs], self.g_temp[:bs], self.g_step, bs)
@@ -804,6 +901,7 @@ class ModelRunner:
             self.graphs[bs] = graph
             torch.cuda.synchronize()
             reset_context()
+        set_done("plain")
         # second set, same pool: the same steps with the penalties and the top-k / top-p / min-p sampler, replayed when some
         # row filters or penalises (the slots are -1 here, so capturing touches no history)
         for bs in reversed(self.graph_bs):
@@ -821,3 +919,23 @@ class ModelRunner:
             self.fgraphs[bs] = graph
             torch.cuda.synchronize()
             reset_context()
+        set_done("filtered")
+        # third set, same pool: the second set's step plus the logprob kernels, replayed when some row wants logprobs (k is
+        # -1 in every row here, so capturing computes nothing)
+        for bs in reversed(self.graph_bs):
+            set_context(False, slot_mapping=self.g_slot[:bs], context_lens=self.g_ctx[:bs], block_tables=self.g_bt[:bs])
+            args = (self.g_ids[:bs], self.g_pos[:bs], self.g_temp[:bs], self.g_step, bs)
+            kw = dict(filters=(self.g_topk[:bs], self.g_topp[:bs], self.g_minp[:bs]),
+                      penalties=(self.g_pslot[:bs], self.g_prep[:bs], self.g_pfreq[:bs], self.g_ppres[:bs], self.g_ids[:bs]),
+                      logprobs=self.g_lpk[:bs])
+            self._forward_and_sample(*args, **kw)
+            torch.cuda.synchronize()
+            graph = torch.cuda.CUDAGraph()
+            before = ops.LAUNCHES[0]
+            with torch.cuda.graph(graph, self.graph_pool):
+                self._forward_and_sample(*args, **kw)
+            self.lgraph_kernels[bs] = ops.LAUNCHES[0] - before
+            self.lgraphs[bs] = graph
+            torch.cuda.synchronize()
+            reset_context()
+        set_done("logprobs")

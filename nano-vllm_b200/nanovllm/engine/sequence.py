@@ -28,7 +28,8 @@ class Sequence:
     __slots__ = ("seq_id", "status", "token_ids", "last_token", "num_tokens", "num_prompt_tokens",
                  "num_cached_tokens", "num_scheduled_tokens", "is_prefill", "block_table",
                  "temperature", "max_tokens", "ignore_eos", "top_k", "top_p", "min_p",
-                 "presence_penalty", "frequency_penalty", "repetition_penalty", "penalised")
+                 "presence_penalty", "frequency_penalty", "repetition_penalty", "penalised",
+                 "logprobs_k", "logprob_rows")
 
     def __init__(self, token_ids: list[int], sampling_params: SamplingParams = _DEFAULT_SP):
         if not token_ids:
@@ -52,6 +53,10 @@ class Sequence:
         self.frequency_penalty = sampling_params.frequency_penalty
         self.repetition_penalty = sampling_params.repetition_penalty
         self.penalised = sampling_params.penalised
+        # requested top-k logprobs (-1: off) and, when on, one packed row per completion token (ops.LOGPROB_OUT_WORDS int32:
+        # the sampled token, the top k, their logprobs and the rank), appended as the token's value arrives
+        self.logprobs_k = -1 if sampling_params.logprobs is None else sampling_params.logprobs
+        self.logprob_rows = None if sampling_params.logprobs is None else []
 
     def __len__(self) -> int:
         return self.num_tokens

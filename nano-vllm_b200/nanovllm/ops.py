@@ -398,6 +398,124 @@ def penalty_apply(logits: torch.Tensor, history: torch.Tensor, lengths: torch.Te
     return logits
 
 
+# ---- per-token logprobs of the raw logits (csrc/logprobs.cu) ------------------------------------------------------------
+LOGPROB_MAX_K = 20
+LOGPROB_ROW_WORDS = 8                      # int64 workspace words per row (include/b200_paged_attn.h)
+# one packed output row (int32 words): ids[0..20] (sampled token, then the top k), logprobs[21..41] (fp32 bits), rank[42]
+LOGPROB_OUT_WORDS = 2 * (LOGPROB_MAX_K + 1) + 1
+LOGPROB_LP_COL = LOGPROB_MAX_K + 1
+LOGPROB_RANK_COL = 2 * (LOGPROB_MAX_K + 1)
+
+
+def logprob_workspace(rows: int, device="cuda") -> torch.Tensor:
+    """Zeroed logprob workspace for up to ``rows`` rows (every ``logprobs_finish`` leaves it zero again)."""
+    n = nat.load().b200_logprob_workspace_words(rows)
+    if n <= 0:
+        raise nat.B200Error("bad logprob workspace row count")
+    return torch.zeros(n, dtype=torch.int64, device=device)
+
+
+def logprob_words(workspace: torch.Tensor, rows: int, lo: int, hi: int) -> torch.Tensor:
+    """Words [lo, hi) of every row of the workspace, a [rows, hi - lo] strided view."""
+    return workspace[:rows * LOGPROB_ROW_WORDS].view(rows, LOGPROB_ROW_WORDS)[:, lo:hi]
+
+
+def _logprob_args(logits: torch.Tensor, k: torch.Tensor, workspace: torch.Tensor):
+    assert logits.dim() == 2 and logits.stride(1) == 1 and logits.is_cuda
+    if logits.dtype == torch.float32:
+        nat.check(-2)                               # B200_EUNSUPPORTED: the logprob kernels read bf16 logits only
+    _need(logits, torch.bfloat16, "logits"); _need(k, torch.int32, "k"); _need(workspace, torch.int64, "workspace")
+    rows = logits.shape[0]
+    assert k.numel() >= rows and workspace.numel() >= rows * LOGPROB_ROW_WORDS, "logprob workspace too small"
+    return rows, logits.shape[1]
+
+
+def logprobs_topk(logits: torch.Tensor, k: torch.Tensor, workspace: torch.Tensor, topk_keys: torch.Tensor,
+                  index_offset: int = 0, reduce=None) -> None:
+    """Before the penalties: each row's top max(k, 1) keys into ``topk_keys`` (int64 [rows, 20]) and its maximum into the
+    workspace, then ``reduce(words, "max")`` of that word when ``reduce`` is given (vocab parallelism)."""
+    rows, vocab = _logprob_args(logits, k, workspace)
+    _need(topk_keys, torch.int64, "topk_keys")
+    assert topk_keys.is_contiguous() and topk_keys.numel() >= rows * LOGPROB_MAX_K
+    nat.check(nat.load().b200_logprob_topk(logits.data_ptr(), logits.stride(0), k.data_ptr(), rows, vocab, index_offset,
+                                           workspace.data_ptr(), topk_keys.data_ptr(), _stream()))
+    if reduce is not None:
+        reduce(logprob_words(workspace, rows, 0, 1), "max")
+
+
+def logprob_saved_buffer(rows: int, capacity: int, device="cuda") -> torch.Tensor:
+    """Scratch of ``logprobs_save``: int64 [rows, capacity + 1] (capacity = the penalty history's)."""
+    return torch.empty(rows, capacity + 1, dtype=torch.int64, device=device)
+
+
+def logprobs_save(logits: torch.Tensor, k: torch.Tensor, workspace: torch.Tensor, saved: torch.Tensor, history: torch.Tensor,
+                  lengths: torch.Tensor, slots: torch.Tensor, pending: torch.Tensor | None = None,
+                  index_offset: int = 0) -> None:
+    """Before ``penalty_apply`` on the same arguments: keep the raw value of every logit it will rewrite."""
+    rows, vocab = _logprob_args(logits, k, workspace)
+    _need(saved, torch.int64, "saved"); _need(history, torch.int64, "history"); _need(lengths, torch.int32, "lengths")
+    _need(slots, torch.int32, "slots")
+    if pending is not None:
+        _need(pending, torch.int64, "pending")
+    num_slots, capacity = history.shape
+    assert saved.is_contiguous() and saved.numel() >= rows * (capacity + 1)
+    nat.check(nat.load().b200_logprob_save(logits.data_ptr(), logits.stride(0), k.data_ptr(), rows, vocab, index_offset,
+                                           history.data_ptr(), lengths.data_ptr(), num_slots, capacity, slots.data_ptr(),
+                                           _ptr(pending), workspace.data_ptr(), saved.data_ptr(), _stream()))
+
+
+def logprobs_finish(logits: torch.Tensor, k: torch.Tensor, tokens: torch.Tensor, workspace: torch.Tensor,
+                    topk_keys: torch.Tensor, out: torch.Tensor, index_offset: int = 0, saved: torch.Tensor | None = None,
+                    capacity: int = 0, reduce=None, gather=None) -> torch.Tensor:
+    """After the token ids ``tokens`` (int64 [rows]) are known: restore the saved logits (``saved`` from
+    ``logprobs_save``, None when no row was penalised), count the rank, sum the softmax mass and write one packed row per
+    logprob row into ``out`` (int32 [rows, LOGPROB_OUT_WORDS]).  Under vocab parallelism ``reduce(words, op)`` all-reduces
+    the words each launch wrote and ``gather(topk_keys)`` returns every rank's keys as one [world, rows, 20] tensor."""
+    rows, vocab = _logprob_args(logits, k, workspace)
+    _need(tokens, torch.int64, "tokens"); _need(out, torch.int32, "out")
+    assert out.dim() == 2 and out.stride(1) == 1 and out.shape[0] >= rows and out.shape[1] >= LOGPROB_OUT_WORDS
+    lib = nat.load()
+    if saved is not None:
+        _need(saved, torch.int64, "saved")
+        assert saved.numel() >= rows * (capacity + 1)
+    nat.check(lib.b200_logprob_restore(logits.data_ptr(), logits.stride(0), k.data_ptr(), rows, vocab, index_offset,
+                                       tokens.data_ptr(), workspace.data_ptr(), _ptr(saved), capacity, _stream()))
+    if reduce is not None:
+        reduce(logprob_words(workspace, rows, 1, 2), "max")
+    nat.check(lib.b200_logprob_rank(logits.data_ptr(), logits.stride(0), k.data_ptr(), rows, vocab, workspace.data_ptr(),
+                                    _stream()))
+    if reduce is not None:
+        reduce(logprob_words(workspace, rows, 2, 4), "sum")
+    mine = topk_keys.view(-1)[:rows * LOGPROB_MAX_K]
+    keys = mine if gather is None else gather(mine)
+    sources = keys.numel() // (rows * LOGPROB_MAX_K)
+    lps = out[:, LOGPROB_LP_COL:].view(torch.float32)
+    nat.check(lib.b200_logprob_finish(k.data_ptr(), rows, tokens.data_ptr(), keys.data_ptr(), sources, workspace.data_ptr(),
+                                      out.data_ptr(), lps.data_ptr(), out[:, LOGPROB_RANK_COL:].data_ptr(), out.stride(0),
+                                      _stream()))
+    return out
+
+
+def logprobs(logits: torch.Tensor, k: torch.Tensor, tokens: torch.Tensor, workspace: torch.Tensor | None = None,
+             out: torch.Tensor | None = None, index_offset: int = 0) -> torch.Tensor:
+    """Logprobs of unpenalised bf16 logits [rows, vocab] for the sampled ``tokens``, unsharded: ``logprobs_topk`` then
+    ``logprobs_finish``.  Returns the packed int32 [rows, LOGPROB_OUT_WORDS] rows (``unpack_logprobs`` reads them)."""
+    rows = logits.shape[0]
+    if workspace is None:
+        workspace = logprob_workspace(rows, device=logits.device)
+    if out is None:
+        out = torch.zeros(rows, LOGPROB_OUT_WORDS, dtype=torch.int32, device=logits.device)
+    keys = torch.empty(rows, LOGPROB_MAX_K, dtype=torch.int64, device=logits.device)
+    logprobs_topk(logits, k, workspace, keys, index_offset)
+    return logprobs_finish(logits, k, tokens, workspace, keys, out, index_offset)
+
+
+def unpack_logprobs(rows, k: int):
+    """One packed row (numpy int32 [LOGPROB_OUT_WORDS] or [n, LOGPROB_OUT_WORDS]) -> (ids [.., 1 + k], fp32 logprobs
+    [.., 1 + k], rank [..]); column 0 is the sampled token, 1.. the top k."""
+    return (rows[..., :1 + k], rows[..., LOGPROB_LP_COL:LOGPROB_LP_COL + 1 + k].view("float32"), rows[..., LOGPROB_RANK_COL])
+
+
 # ---- decode-size projections on wgmma (csrc/linear_tc.cu) -------------------------------------------------------------
 EPI_BF16, EPI_SILU, EPI_PARTIAL = 0, 1, 2
 

@@ -18,13 +18,29 @@ keyword-or-positional arguments after ``min_p`` and attributes like the fields, 
 pickling, ``copy.copy`` and ``copy.replace`` include them.  ``dataclasses.replace`` and ``dataclasses.asdict`` only see the
 dataclass fields, so they drop the penalties (``replace`` resets them to off): use ``sp.replace(**changes)`` and
 ``sp.as_dict()`` instead.
+
+Last, ``logprobs`` (DESIGN.md 3.3.2): None (off) or k in [0, 20].  Each generated token then gets the log_softmax of the raw
+logits (before penalties, temperature and filters) for the sampled token, with its rank, and for the k most likely
+tokens; ``generate()`` returns them as one ``{token_id: Logprob}`` dict per token.  It is handled like the penalties, but
+``as_dict()`` and ``repr`` list it only when it is set.
 """
 import math
 from dataclasses import dataclass
 
+MAX_LOGPROBS = 20
+# vLLM parameters this engine does not implement; any value but "off" is refused
+_UNSUPPORTED = {"prompt_logprobs": None, "logprob_token_ids": None, "logprobs_mode": "raw_logprobs"}
+
+
+@dataclass(frozen=True, slots=True)
+class Logprob:
+    """One entry of a per-token logprobs dict: the log-probability under the raw logits and the rank (1 = most likely)."""
+    logprob: float
+    rank: int
+
 
 class _Penalties:
-    __slots__ = ("presence_penalty", "frequency_penalty", "repetition_penalty")
+    __slots__ = ("presence_penalty", "frequency_penalty", "repetition_penalty", "logprobs")
 
 
 @dataclass(slots=True, init=False, repr=False, eq=False)
@@ -38,7 +54,12 @@ class SamplingParams(_Penalties):
 
     def __init__(self, temperature: float = 1.0, max_tokens: int = 64, ignore_eos: bool = False, top_k: int = -1,
                  top_p: float = 1.0, min_p: float = 0.0, presence_penalty: float = 0.0, frequency_penalty: float = 0.0,
-                 repetition_penalty: float = 1.0):
+                 repetition_penalty: float = 1.0, logprobs: int | None = None, **unsupported):
+        for name, value in unsupported.items():
+            if name not in _UNSUPPORTED:
+                raise TypeError(f"SamplingParams got an unexpected keyword argument {name!r}")
+            if value != _UNSUPPORTED[name]:
+                raise ValueError(f"{name}={value!r} is not supported (only {_UNSUPPORTED[name]!r})")
         self.temperature = temperature
         self.max_tokens = max_tokens
         self.ignore_eos = ignore_eos
@@ -48,6 +69,7 @@ class SamplingParams(_Penalties):
         self.presence_penalty = presence_penalty
         self.frequency_penalty = frequency_penalty
         self.repetition_penalty = repetition_penalty
+        self.logprobs = logprobs
         self.__post_init__()
 
     def __post_init__(self):
@@ -67,20 +89,27 @@ class SamplingParams(_Penalties):
             raise ValueError("frequency_penalty must be in [-2, 2] (0 = off)")
         if not (math.isfinite(self.repetition_penalty) and self.repetition_penalty > 0.0):
             raise ValueError("repetition_penalty must be finite and > 0 (1 = off)")
+        lp = self.logprobs
+        if lp is not None and (type(lp) is bool or not isinstance(lp, int) or not 0 <= lp <= MAX_LOGPROBS):
+            raise ValueError(f"logprobs must be None (off) or an int in [0, {MAX_LOGPROBS}] (the full vocabulary, -1, "
+                             "is not supported)")
 
     _NAMES = ("temperature", "max_tokens", "ignore_eos", "top_k", "top_p", "min_p", "presence_penalty",
               "frequency_penalty", "repetition_penalty")
 
     def _values(self) -> tuple:
-        return tuple(getattr(self, n) for n in self._NAMES)
+        return tuple(getattr(self, n) for n in self._NAMES) + (self.logprobs,)
 
     def as_dict(self) -> dict:
-        """Every parameter by name, penalties included (``dataclasses.asdict`` omits them)."""
-        return dict(zip(self._NAMES, self._values()))
+        """Every parameter by name, penalties included (``dataclasses.asdict`` omits them); logprobs only when set."""
+        d = {n: getattr(self, n) for n in self._NAMES}
+        if self.logprobs is not None:
+            d["logprobs"] = self.logprobs
+        return d
 
     def replace(self, **changes) -> "SamplingParams":
         """A validated copy with `changes` applied, penalties kept (``dataclasses.replace`` resets them)."""
-        unknown = set(changes) - set(self._NAMES)
+        unknown = set(changes) - set(self._NAMES) - {"logprobs"}
         if unknown:
             raise TypeError(f"unknown sampling parameters: {sorted(unknown)}")
         return SamplingParams(**{**self.as_dict(), **changes})
