@@ -16,8 +16,9 @@ import torch
 
 from gpu_helpers import record
 from kv_fp8_ref import dequantize_e4m3, quantize_e4m3
-from test_gpu_dispatch_edges import (D, EPS, SCALE, assert_close_bf16, assert_ran, assert_rows_close, build_paged, cu,
-                                     decode64, edge_rows, launched, mixed_lens, norm_weight, prefill64, randn)
+from test_gpu_dispatch_edges import (D, EPS, SCALE, assert_close_bf16, assert_ran, assert_rows_close, assert_vectors_close,
+                                     build_paged, cu, decode64, edge_rows, launched, mixed_lens, norm_weight, prefill64,
+                                     randn)
 
 pytestmark = pytest.mark.gpu
 
@@ -165,11 +166,11 @@ def test_decode_fp8(ops, G, bs):
     got, names = launched(lambda: ops.paged_decode(0, q, c.tables, ctx, SCALE))
     assert_ran(names, f"paged_decode_mma_fp8_kernel<{G}>", f"decode fp8 G={G}")
     want = decode64(q, K, V, lens, c.tables)
-    assert_close_bf16(got, want, f"decode fp8 G={G} bs={bs} batch {batch}")
+    assert_vectors_close(got, want, f"decode fp8 G={G} bs={bs} batch {batch}")
     assert_rows_close(got, want, [i for i in edge_rows(batch, extra=range(16)) if lens[i]], f"decode fp8 G={G}")
     assert (got[ctx == 0] == 0).all(), "zero-context rows are exactly zero"
     for b in (1, 3, 256):                                   # smaller batches through the same workspace
-        assert_close_bf16(ops.paged_decode(0, q[:b], c.tables[:b], ctx[:b], SCALE), want[:b], f"decode fp8 G={G} batch {b}")
+        assert_vectors_close(ops.paged_decode(0, q[:b], c.tables[:b], ctx[:b], SCALE), want[:b], f"decode fp8 G={G} batch {b}")
     again = ops.paged_decode(0, q, c.tables, ctx, SCALE)
     nat.handle().workspace = None
     fresh = ops.paged_decode(0, q, c.tables, ctx, SCALE)
@@ -199,6 +200,7 @@ def test_decode_fp8_long_context(ops, G, nseq):
     got, names = launched(lambda: ops.paged_decode(0, q, c.tables, ctx, SCALE))
     assert_ran(names, f"paged_decode_mma_fp8_kernel<{G}>", f"decode fp8 G={G} context 40960")
     want = decode64(q, K, V, lens, c.tables)
+    assert_vectors_close(got, want, f"decode fp8 G={G} {nseq} x 40960")
     for i in range(nseq):
         assert_close_bf16(got[i], want[i], f"decode fp8 G={G} sequence {i}")
 
@@ -212,18 +214,18 @@ def test_bind_bf16_fp8_bf16_one_process(ops):
     ctx = torch.tensor(lens, dtype=torch.int32, device="cuda")
     a = build_paged(lens, bs, hkv, seed=11)
     ops.bind_kv_cache(a.kv)
-    assert_close_bf16(ops.paged_decode(0, q, a.tables, ctx, SCALE), decode64(q, a.K, a.V, lens, a.tables), "bf16 bind 1")
+    assert_vectors_close(ops.paged_decode(0, q, a.tables, ctx, SCALE), decode64(q, a.K, a.V, lens, a.tables), "bf16 bind 1")
     b = build_paged(lens, bs, hkv, seed=12)
     kv8, K, V = fp8_paged(b, 1.0, 1.0)
     ops.bind_kv_cache(kv8)
     got, names = launched(lambda: ops.paged_decode(0, q, b.tables, ctx, SCALE))
     assert_ran(names, f"paged_decode_mma_fp8_kernel<{G}>", "fp8 bind")
-    assert_close_bf16(got, decode64(q, K, V, lens, b.tables), "fp8 bind")
+    assert_vectors_close(got, decode64(q, K, V, lens, b.tables), "fp8 bind")
     c = build_paged(lens, bs, hkv, seed=13)
     ops.bind_kv_cache(c.kv)
     got, names = launched(lambda: ops.paged_decode(0, q, c.tables, ctx, SCALE))
     assert_ran(names, f"paged_decode_mma_kernel<{G}>", "bf16 bind 2")
-    assert_close_bf16(got, decode64(q, c.K, c.V, lens, c.tables), "bf16 bind 2")
+    assert_vectors_close(got, decode64(q, c.K, c.V, lens, c.tables), "bf16 bind 2")
 
 
 def test_fp8_refusals(ops):
@@ -295,7 +297,7 @@ def test_paged_prefill_fp8(ops, case):
     cache = SimpleNamespace(K=logical(kv8, 0, 0, ks).to(torch.bfloat16), V=logical(kv8, 0, 1, vs).to(torch.bfloat16),
                             tables=c.tables)
     want = prefill64(q, cq, ck, cache=cache)
-    assert_close_bf16(got, want, f"prefill fp8 {case}")
+    assert_vectors_close(got, want, f"prefill fp8 {case}")
     ends = (torch.tensor(lq).cumsum(0) - 1).tolist()
     assert_rows_close(got, want, edge_rows(sum(lq), extra=ends), f"prefill fp8 {case}")
 
