@@ -368,6 +368,22 @@ int b200_logprob_finish(const int32_t* k, int rows, const int64_t* tokens, const
 int b200_linear(const void* x, int64_t x_stride0, const void* w, void* out, int64_t out_stride0, int rows,
                 int n_out, int k, int epilogue, int block_n, int k_splits, int flags, void* stream);
 
+/* ---- block-scaled FP8 projections (Qwen / DeepSeek "fp8" checkpoints with weight_block_size [128, 128]) -------------
+ *
+ * b200_quant_fp8: dynamic activation quantization of x [rows, k] bf16 (row stride x_stride0, k % 128 == 0): per row and
+ *   128-column group g, s = max(amax_g, 1e-10) / 448 and q = e4m3_satfinite_rn(x / s) (IEEE fp32 divisions);
+ *   q [rows, k] e4m3 bytes (row stride q_stride0), scales [rows, k / 128] fp32 (row stride scales_stride0).
+ * b200_linear_fp8: b200_linear on e4m3 operands.  x [rows, k] e4m3 (x_stride0 % 16 == 0) with x_scale from
+ *   b200_quant_fp8; w [w_rows, k] e4m3 contiguous with w_scale [w_rows / 128, k / 128] fp32 contiguous (w_rows = n_out,
+ *   2 * n_out for epilogue 1); k and n_out multiples of 128.  Each 128-wide block of K is summed by the tensor cores into
+ *   a fresh fp32 partial, then acc += partial * (x_scale[row, kb] * w_scale[nb, kb]).  epilogue, k_splits and flags as
+ *   b200_linear (k_splits divides k / 128); block_n one of 16 (not for epilogue 1), 32, 64. */
+int b200_quant_fp8(const void* x, int64_t x_stride0, void* q, int64_t q_stride0, float* scales, int64_t scales_stride0,
+                   int rows, int k, void* stream);
+int b200_linear_fp8(const void* x, int64_t x_stride0, const float* x_scale, int64_t x_scale_stride0, const void* w,
+                    const float* w_scale, void* out, int64_t out_stride0, int rows, int n_out, int k, int epilogue,
+                    int block_n, int k_splits, int flags, void* stream);
+
 /* (opt-in) ParallelLMHead.forward + Sampler.forward in one pass (layers/embed_head.py:56-66, layers/sampler.py:7-12):
  * logits = bf16(hidden lm_head^T) are produced tile by tile in registers, scored exactly as b200_sample scores
  * them (same RNG keyed by (seed, step, row, vocabulary id); temperature 0 = greedy, lowest index on ties) and

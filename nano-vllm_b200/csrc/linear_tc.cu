@@ -24,6 +24,8 @@
 #include <type_traits>
 #include <unordered_map>
 
+#include <cuda_fp8.h>
+
 #include "sample_common.cuh"
 #include "tc_common.cuh"
 
@@ -103,9 +105,20 @@ __device__ __forceinline__ void release_slot(uint32_t empty_bar, int lane) {
     }
 }
 
-template <int BN, int EPI, bool DEEP, int CL>
+// Block-scaled FP8 operands (linear_tc_kernel<..., true>): x and W are e4m3, one fp32 scale per row of x and 128 columns, and one
+// per 128 x 128 block of W.  A ring slot of 128 bytes per row is then exactly one scale block of K.
+struct Fp8Scales {
+    const float* x_scale;     // [rows, k / 128], row stride xs_stride
+    int64_t xs_stride;
+    const float* w_scale;     // [w_rows / 128, k / 128] contiguous
+    int ws_cols;              // k / 128
+};
+
+// FP8: x and W are e4m3 (b200_linear_fp8).  Both tensor maps then describe the fp8 bytes as bf16 pairs, so a 64-"column"
+// box is one 128-byte row of 128 e4m3 elements and the producer below serves both operand types coordinate for coordinate.
+template <int BN, int EPI, bool DEEP, int CL, bool FP8>
 __global__ void __launch_bounds__(L_THREADS, 1)
-linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const LinParams p) {
+linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const LinParams p, const Fp8Scales fs) {
     using C = Cfg<BN, DEEP>;
     constexpr uint16_t CL_MASK = (uint16_t)((1u << CL) - 1);
     constexpr int X_ROWS = LM / CL;                            // rows of x this CTA fetches (and multicasts when CL > 1)
@@ -182,6 +195,77 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
         // the row-half decision is taken once, outside the MMA loop, so that every wgmma sequence is straight-line code
         auto consume = [&](auto two) {
             constexpr bool TWO = decltype(two)::value;
+            if constexpr (FP8) {
+                // One slot = one 128-wide scale block of K: its four k32 MMAs accumulate a fresh fp32 partial, which is
+                // promoted into acc with the block's scales once it has retired (fp8 wgmma accumulates with reduced
+                // precision inside one instruction chain, so chains stay one scale block long).
+                asm volatile("griddepcontrol.wait;" ::: "memory");   // x_scale is the previous kernel's output
+                float part[2][BN / 2];
+                const int g = lane >> 2;
+                const int wrow = EPI == EPI_SILU ? blockIdx.x * BOUT : blockIdx.x * BN;
+                const float* ws_gate = fs.w_scale + (int64_t)(wrow / 128) * fs.ws_cols;
+                const float* ws_up = fs.w_scale + (int64_t)((p.up_row0 + wrow) / 128) * fs.ws_cols;
+                // Scales are read SPF blocks ahead into registers (slot j of the unrolled loop holds block i0 + j), so that
+                // their L2 latency hides under the MMAs of the blocks in between instead of stalling every block.
+                constexpr int SPF = 4;
+                float sx[SPF][2][2], swg[SPF], swu[SPF];
+                auto load_scales = [&](float (&x)[2][2], float& wg, float& wu, int i) {
+                    if (i >= nk) return;
+                    const int kb = kt0 + i;
+                    wg = ws_gate[kb];
+                    wu = EPI == EPI_SILU ? ws_up[kb] : wg;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int r = 0; r < 2; ++r) {
+                            const int row = m0 + 64 * h + 16 * warp + g + 8 * r;      // rows past `rows` are never stored
+                            x[h][r] = row < p.rows ? fs.x_scale[(int64_t)row * fs.xs_stride + kb] : 0.f;
+                        }
+                };
+#pragma unroll
+                for (int j = 0; j < SPF; ++j) load_scales(sx[j], swg[j], swu[j], j);
+                for (int i0 = 0; i0 < nk; i0 += SPF) {
+#pragma unroll
+                    for (int j = 0; j < SPF; ++j) {
+                        const int i = i0 + j;
+                        if (i >= nk) break;
+                        const int slot = i % S, round = i / S;
+                        mbar_wait(bars + slot * 8, round & 1);
+                        const uint32_t xs = base + slot * C::STAGE, ws = xs + X_TILE;
+                        wg_fence();
+#pragma unroll
+                        for (int ks = 0; ks < 4; ++ks) {
+                            const uint64_t bdesc = make_desc(ws + ks * 32, 16, 1024);
+                            wgmma_ss_e4m3<BN>(part[0], make_desc(xs + ks * 32, 16, 1024), bdesc, ks > 0 ? 1u : 0u);
+                            if constexpr (TWO) wgmma_ss_e4m3<BN>(part[1], make_desc(xs + X_HALF + ks * 32, 16, 1024), bdesc, ks > 0 ? 1u : 0u);
+                        }
+                        wg_commit();
+                        float sg[2][2], su[2][2];
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+#pragma unroll
+                            for (int r = 0; r < 2; ++r) {
+                                sg[h][r] = sx[j][h][r] * swg[j];
+                                su[h][r] = sx[j][h][r] * swu[j];
+                            }
+                        load_scales(sx[j], swg[j], swu[j], i + SPF);
+                        wg_wait<0>();
+                        acc_fence(part[0]);
+                        if constexpr (TWO) acc_fence(part[1]);
+                        release_slot<CL>(bars + (S + slot) * 8, lane);
+#pragma unroll
+                        for (int h = 0; h < (TWO ? 2 : 1); ++h)
+#pragma unroll
+                            for (int c = 0; c < BN / 8; ++c)
+#pragma unroll
+                                for (int r = 0; r < 2; ++r) {
+                                    const float sc = (EPI == EPI_SILU && c >= BOUT / 8) ? su[h][r] : sg[h][r];
+                                    acc[h][4 * c + 2 * r] = fmaf(part[h][4 * c + 2 * r], sc, acc[h][4 * c + 2 * r]);
+                                    acc[h][4 * c + 2 * r + 1] = fmaf(part[h][4 * c + 2 * r + 1], sc, acc[h][4 * c + 2 * r + 1]);
+                                }
+                    }
+                }
+            } else {
             for (int i = 0; i < nk; ++i) {
                 const int slot = i % S, round = i / S;
                 mbar_wait(bars + slot * 8, round & 1);
@@ -198,12 +282,13 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
                 if (i > 0) release_slot<CL>(bars + (S + (i - 1) % S) * 8, lane);
             }
             wg_wait<0>();
+            }
         };
         if (two_halves) consume(std::true_type{});
         else consume(std::false_type{});
         acc_fence(acc[0]);
         acc_fence(acc[1]);
-        if (nk > 0) release_slot<CL>(bars + (S + (nk - 1) % S) * 8, lane);
+        if (!FP8 && nk > 0) release_slot<CL>(bars + (S + (nk - 1) % S) * 8, lane);
     }
 
     // ---- epilogue (warpgroup 0): acc[h][4c + 2r + e] = D[64 h + 16 warp + g + 8 r][8 c + 2 qd + e] ---------------------
@@ -266,6 +351,27 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
     }
     __syncwarp();                                  // the producer warp's lanes reconverge before the .aligned cluster barrier
     if constexpr (CL > 1) cluster_sync_all();      // nobody leaves while a peer may still signal its barriers
+}
+
+// Dynamic activation quantization: per row and 128-column group, s = max(amax, 1e-10) / 448 and q = e4m3_satfinite_rn(x / s),
+// both IEEE fp32 divisions.  One warp per (row, group); lane j holds columns 4j .. 4j + 3.
+__global__ void __launch_bounds__(256) quant_fp8_kernel(const __nv_bfloat16* __restrict__ x, int64_t x_stride, uint8_t* q, int64_t q_stride,
+                                                        float* scales, int64_t s_stride, int rows, int groups) {
+    B200_PDL_SYNC();
+    const int64_t w = ((int64_t)blockIdx.x * 256 + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (w >= (int64_t)rows * groups) return;
+    const int64_t row = w / groups;
+    const int grp = (int)(w - row * groups);
+    const uint2 raw = *reinterpret_cast<const uint2*>(x + row * x_stride + grp * 128 + lane * 4);
+    const __nv_bfloat162 b01 = *reinterpret_cast<const __nv_bfloat162*>(&raw.x), b23 = *reinterpret_cast<const __nv_bfloat162*>(&raw.y);
+    const float v[4] = {__low2float(b01), __high2float(b01), __low2float(b23), __high2float(b23)};
+    const float amax = warp_max(fmaxf(fmaxf(fabsf(v[0]), fabsf(v[1])), fmaxf(fabsf(v[2]), fabsf(v[3]))));
+    const float s = __fdiv_rn(fmaxf(amax, 1e-10f), 448.f);
+    const __nv_fp8x2_storage_t lo = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(v[0], s), __fdiv_rn(v[1], s)), __NV_SATFINITE, __NV_E4M3);
+    const __nv_fp8x2_storage_t hi = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(v[2], s), __fdiv_rn(v[3], s)), __NV_SATFINITE, __NV_E4M3);
+    *reinterpret_cast<uint32_t*>(q + row * q_stride + grp * 128 + lane * 4) = (uint32_t)lo | ((uint32_t)hi << 16);
+    if (lane == 0) scales[row * s_stride + grp] = s;
 }
 
 // RMSNorm.add_rms_forward (layers/layernorm.py:28-40) on a split-K projection: x = bf16(sum over splits, in order).
@@ -372,13 +478,13 @@ bool b200_cached_tensor_map(CUtensorMap* out, const void* base, uint64_t cols, u
 
 namespace {
 
-template <int BN, int EPI, bool DEEP, int CL>
-int launch_linear(const CUtensorMap& tx, const CUtensorMap& tw, LinParams prm, dim3 grid, bool pdl, cudaStream_t stream) {
+template <int BN, int EPI, bool DEEP, int CL, bool FP8>
+int launch_linear(const CUtensorMap& tx, const CUtensorMap& tw, LinParams prm, const Fp8Scales& fs, dim3 grid, bool pdl, cudaStream_t stream) {
     using C = Cfg<BN, DEEP>;
     if (prm.stages <= 0 || prm.stages > C::STAGES) prm.stages = C::STAGES;      // 0: this configuration's full ring
     if (prm.stages < 2) prm.stages = 2;
     static B200SmemOptIn optin;
-    if (cudaError_t e = optin.ensure(linear_tc_kernel<BN, EPI, DEEP, CL>, C::SMEM); e != cudaSuccess) {
+    if (cudaError_t e = optin.ensure(linear_tc_kernel<BN, EPI, DEEP, CL, FP8>, C::SMEM); e != cudaSuccess) {
         b200_tls_cuda_error() = cudaGetErrorString(e);
         return B200_ECUDA;
     }
@@ -403,25 +509,27 @@ int launch_linear(const CUtensorMap& tx, const CUtensorMap& tw, LinParams prm, d
     }
     cfg.attrs = attr;
     cfg.numAttrs = na;
-    if (cudaLaunchKernelEx(&cfg, linear_tc_kernel<BN, EPI, DEEP, CL>, tx, tw, prm) != cudaSuccess) return B200_ECUDA;
+    if (cudaLaunchKernelEx(&cfg, linear_tc_kernel<BN, EPI, DEEP, CL, FP8>, tx, tw, prm, fs) != cudaSuccess) return B200_ECUDA;
     return B200_OK;
 }
 
-template <int EPI, bool DEEP, int CL>
-int dispatch_bn(int bn, const CUtensorMap& tx, const CUtensorMap& tw, const LinParams& prm, dim3 grid, bool pdl, cudaStream_t stream) {
+// FP8 keeps a second fp32 accumulator (the partial of the current scale block), so block_n 128 would spill: 16 .. 64 only
+template <int EPI, bool DEEP, int CL, bool FP8>
+int dispatch_bn(int bn, const CUtensorMap& tx, const CUtensorMap& tw, const LinParams& prm, const Fp8Scales& fs, dim3 grid, bool pdl, cudaStream_t stream) {
     switch (bn) {
-        case 16: if constexpr (EPI == EPI_SILU) return B200_EUNSUPPORTED; else return launch_linear<16, EPI, DEEP, CL>(tx, tw, prm, grid, pdl, stream);
-        case 32: return launch_linear<32, EPI, DEEP, CL>(tx, tw, prm, grid, pdl, stream);
-        case 64: return launch_linear<64, EPI, DEEP, CL>(tx, tw, prm, grid, pdl, stream);
-        case 128: return launch_linear<128, EPI, DEEP, CL>(tx, tw, prm, grid, pdl, stream);
+        case 16: if constexpr (EPI == EPI_SILU) return B200_EUNSUPPORTED; else return launch_linear<16, EPI, DEEP, CL, FP8>(tx, tw, prm, fs, grid, pdl, stream);
+        case 32: return launch_linear<32, EPI, DEEP, CL, FP8>(tx, tw, prm, fs, grid, pdl, stream);
+        case 64: return launch_linear<64, EPI, DEEP, CL, FP8>(tx, tw, prm, fs, grid, pdl, stream);
+        case 128: if constexpr (FP8) return B200_EUNSUPPORTED; else return launch_linear<128, EPI, DEEP, CL, FP8>(tx, tw, prm, fs, grid, pdl, stream);
         default: return B200_EUNSUPPORTED;
     }
 }
-template <int EPI>
-int dispatch_depth(bool deep, int cluster, int bn, const CUtensorMap& tx, const CUtensorMap& tw, const LinParams& prm, dim3 grid, bool pdl, cudaStream_t stream) {
-    if (cluster == 2) return dispatch_bn<EPI, true, 2>(bn, tx, tw, prm, grid, pdl, stream);       // multicast variants: deep ring only
-    if (cluster == 4) return dispatch_bn<EPI, true, 4>(bn, tx, tw, prm, grid, pdl, stream);
-    return deep ? dispatch_bn<EPI, true, 1>(bn, tx, tw, prm, grid, pdl, stream) : dispatch_bn<EPI, false, 1>(bn, tx, tw, prm, grid, pdl, stream);
+template <int EPI, bool FP8 = false>
+int dispatch_depth(bool deep, int cluster, int bn, const CUtensorMap& tx, const CUtensorMap& tw, const LinParams& prm, dim3 grid, bool pdl, cudaStream_t stream,
+                   const Fp8Scales& fs = Fp8Scales{}) {
+    if (cluster == 2) return dispatch_bn<EPI, true, 2, FP8>(bn, tx, tw, prm, fs, grid, pdl, stream);       // multicast variants: deep ring only
+    if (cluster == 4) return dispatch_bn<EPI, true, 4, FP8>(bn, tx, tw, prm, fs, grid, pdl, stream);
+    return deep ? dispatch_bn<EPI, true, 1, FP8>(bn, tx, tw, prm, fs, grid, pdl, stream) : dispatch_bn<EPI, false, 1, FP8>(bn, tx, tw, prm, fs, grid, pdl, stream);
 }
 
 }  // namespace
@@ -529,5 +637,66 @@ extern "C" int b200_add_rmsnorm_partials(const float* partials, int splits, void
     if (cudaLaunchKernelEx(&cfg, add_rmsnorm_partials_kernel, partials, splits, (int64_t)rows * cols, static_cast<__nv_bfloat16*>(residual),
                            static_cast<const __nv_bfloat16*>(weight), static_cast<__nv_bfloat16*>(out), cols, eps) != cudaSuccess)
         return B200_ECUDA;
+    return b200_launch_status(nullptr);
+}
+
+extern "C" int b200_quant_fp8(const void* x, int64_t x_stride0, void* q, int64_t q_stride0, float* scales, int64_t scales_stride0,
+                              int rows, int k, void* stream) {
+    if (!x || !q || !scales || rows < 0 || k <= 0) return B200_EINVAL;
+    if (((uintptr_t)x & 7) || ((uintptr_t)q & 3) || ((uintptr_t)scales & 3) || (x_stride0 % 4) || (q_stride0 % 4)) return B200_EINVAL;
+    if (k % 128) return B200_EUNSUPPORTED;
+    if (x_stride0 < k || q_stride0 < k || scales_stride0 < k / 128) return B200_EINVAL;
+    if (rows == 0) return B200_OK;
+    const int groups = k / 128;
+    const int64_t blocks = ((int64_t)rows * groups + 7) / 8;
+    if (blocks > 0x7fffffff) return B200_EUNSUPPORTED;
+    B200_LAUNCH((quant_fp8_kernel), (unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream), static_cast<const __nv_bfloat16*>(x),
+                x_stride0, static_cast<uint8_t*>(q), q_stride0, scales, scales_stride0, rows, groups);
+    return b200_launch_status(nullptr);
+}
+
+extern "C" int b200_linear_fp8(const void* x, int64_t x_stride0, const float* x_scale, int64_t x_scale_stride0, const void* w,
+                               const float* w_scale, void* out, int64_t out_stride0, int rows, int n_out, int k, int epilogue,
+                               int block_n, int k_splits, int flags, void* stream) {
+    if (!x || !x_scale || !w || !w_scale || !out || rows < 0 || n_out <= 0 || k <= 0) return B200_EINVAL;
+    if (((uintptr_t)x & 15) || ((uintptr_t)w & 15) || ((uintptr_t)out & 15) || ((uintptr_t)x_scale & 3) || ((uintptr_t)w_scale & 3))
+        return B200_EINVAL;
+    if ((x_stride0 % 16) || (out_stride0 % 8) || x_stride0 < k) return B200_EINVAL;
+    if (epilogue < EPI_BF16 || epilogue > EPI_PARTIAL || k_splits < 1) return B200_EINVAL;
+    if (k % 128 || n_out % 128) return B200_EUNSUPPORTED;                 // whole 128 x 128 scale blocks of W
+    if (x_scale_stride0 < k / 128) return B200_EINVAL;
+    const int k_blocks = k / 128;
+    if (k_blocks % k_splits) return B200_EUNSUPPORTED;
+    if (k_splits > 1 && epilogue != EPI_PARTIAL) return B200_EINVAL;
+    if (block_n != 16 && block_n != 32 && block_n != 64) return B200_EUNSUPPORTED;
+    if (epilogue == EPI_SILU && block_n == 16) return B200_EUNSUPPORTED;
+    const int bout = epilogue == EPI_SILU ? block_n / 2 : block_n;
+    if (rows == 0) return B200_OK;
+    const int w_rows = epilogue == EPI_SILU ? 2 * n_out : n_out;
+    const int cluster = 1 << ((flags >> 2) & 3);
+    if (cluster > 4 || (cluster > 1 && (flags & 2))) return B200_EUNSUPPORTED;
+    if ((n_out / bout) % cluster) return B200_EUNSUPPORTED;
+    // e4m3 bytes described as bf16 pairs: 64 "columns" of a box are one 128-byte row of 128 elements
+    CUtensorMap tx, tw;
+    if (!cached_map(&tx, x, (uint64_t)k / 2, (uint64_t)rows, (uint64_t)x_stride0 / 2, LM / cluster)) return B200_EUNSUPPORTED;
+    if (!cached_map(&tw, w, (uint64_t)k / 2, (uint64_t)w_rows, (uint64_t)k / 2, (uint32_t)bout)) return B200_EUNSUPPORTED;
+    LinParams prm = {};
+    prm.out = out;
+    prm.out_stride = out_stride0;
+    prm.rows = rows;
+    prm.up_row0 = n_out;
+    prm.k_tiles = k_blocks / k_splits;
+    prm.stages = (flags >> 4) & 15;
+    const Fp8Scales fs{x_scale, x_scale_stride0, w_scale, k_blocks};
+    dim3 grid(n_out / bout, (rows + LM - 1) / LM, k_splits);
+    if (grid.y > 65535 || grid.z > 65535) return B200_EUNSUPPORTED;
+    const bool pdl = (flags & 1) != 0;
+    const bool deep = (flags & 2) == 0;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int rc;
+    if (epilogue == EPI_BF16) rc = dispatch_depth<EPI_BF16, true>(deep, cluster, block_n, tx, tw, prm, grid, pdl, st, fs);
+    else if (epilogue == EPI_SILU) rc = dispatch_depth<EPI_SILU, true>(deep, cluster, block_n, tx, tw, prm, grid, pdl, st, fs);
+    else rc = dispatch_depth<EPI_PARTIAL, true>(deep, cluster, block_n, tx, tw, prm, grid, pdl, st, fs);
+    if (rc != B200_OK) return rc;
     return b200_launch_status(nullptr);
 }

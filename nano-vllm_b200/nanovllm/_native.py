@@ -53,6 +53,8 @@ SIGNATURES = {
     "b200_logprob_finish": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i64, _vp]),
     # decode-size projections on wgmma (csrc/linear_tc.cu) and the fused LM head / layer tail experiments
     "b200_linear": (_i, [_vp, _i64, _vp, _vp, _i64, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "b200_quant_fp8": (_i, [_vp, _i64, _vp, _i64, _vp, _i64, _i, _i, _vp]),
+    "b200_linear_fp8": (_i, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "b200_add_rmsnorm_partials": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _f, _i, _vp]),
     "b200_lm_head_sample": (_i, [_vp, _i64, _vp, _i, _i, _i, _vp, _i64, _u64, _u64, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     "b200_layer_tail_workspace_bytes": (_sz, [_i, _i, _i, _i]),

@@ -30,6 +30,7 @@ import torch.nn.functional as F
 from .. import ops
 from ..layers.attention import Attention
 from ..layers.rotary_embedding import build_cos_sin
+from ..utils import fp8 as fp8fmt
 from ..utils.context import get_context
 
 
@@ -43,6 +44,11 @@ class LayerWeights:
     ln2: torch.Tensor
     q_norm: torch.Tensor
     k_norm: torch.Tensor
+    # block-FP8 checkpoints: the four projections above are e4m3 and these are their fp32 [N / 128, K / 128] block scales
+    qkv_s: torch.Tensor | None = None
+    o_s: torch.Tensor | None = None
+    gate_up_s: torch.Tensor | None = None
+    down_s: torch.Tensor | None = None
 
 
 class Qwen3ForCausalLM:
@@ -55,6 +61,7 @@ class Qwen3ForCausalLM:
     def __init__(self, hf_config, tp_rank: int = 0, tp_size: int = 1, device="cuda", max_position: int | None = None):
         c = hf_config
         self.cfg = c
+        self.fp8 = fp8fmt.is_block_fp8(c)          # the checkpoint's quantization_config is the switch (DESIGN.md 3.6)
         self.tp_rank, self.tp_size = tp_rank, tp_size
         self.device = torch.device(device)
         self.hidden = c.hidden_size
@@ -68,6 +75,8 @@ class Qwen3ForCausalLM:
         self.eps = c.rms_norm_eps
         self.q_size = self.num_heads * self.head_dim
         self.kv_size = self.num_kv_heads * self.head_dim
+        if self.fp8:
+            fp8fmt.check_shapes(self.q_size, self.kv_size, self.hidden, self.inter)
         self.tie = bool(getattr(c, "tie_word_embeddings", False))
         # b200_paged_decode_fused folds q/k-norm + RoPE + KV append into the decode kernel (one launch less per
         # layer).  The extra per-segment math lands on warps that are already busy, which costs more than the saved
@@ -130,6 +139,8 @@ class Qwen3ForCausalLM:
         else:
             self.dual_cfg[3], self.dual_cfg[5] = fit(self.q_size, self.dual_cfg[3]), fit(self.inter, self.dual_cfg[5])
         self._dual_state = None
+        if self.fp8:            # the wgmma / layer-tail / two-stream experiments above are bf16-only
+            self.tc_linear = self.tc_gate_up = self.mega_tail = self.dual = False
         if getattr(c, "attention_bias", False):
             raise NotImplementedError("qkv bias (Qwen2-style) is outside the Qwen3 hot path")
         theta = getattr(c, "rope_theta", 1000000.0)
@@ -145,10 +156,17 @@ class Qwen3ForCausalLM:
         self.lm_head = (self.embed[tp_rank * self.vocab_shard:(tp_rank + 1) * self.vocab_shard]
                         if self.tie else e(self.vocab_shard, self.hidden))
         self.norm = e(self.hidden)
-        self.layers = [LayerWeights(e(self.q_size + 2 * self.kv_size, self.hidden), e(self.hidden, self.q_size),
-                                    e(2 * self.inter, self.hidden), e(self.hidden, self.inter),
-                                    e(self.hidden), e(self.hidden), e(self.head_dim), e(self.head_dim))
-                       for _ in range(c.num_hidden_layers)]
+        proj = [(self.q_size + 2 * self.kv_size, self.hidden), (self.hidden, self.q_size), (2 * self.inter, self.hidden),
+                (self.hidden, self.inter)]
+        if self.fp8:
+            q8 = lambda n, k: torch.empty(n, k, dtype=torch.float8_e4m3fn, device=dev)
+            sc = lambda n, k: torch.empty(n // fp8fmt.BLOCK, k // fp8fmt.BLOCK, dtype=torch.float32, device=dev)
+            self.layers = [LayerWeights(*(q8(*p) for p in proj), e(self.hidden), e(self.hidden), e(self.head_dim), e(self.head_dim),
+                                        *(sc(*p) for p in proj))
+                           for _ in range(c.num_hidden_layers)]
+        else:
+            self.layers = [LayerWeights(*(e(*p) for p in proj), e(self.hidden), e(self.hidden), e(self.head_dim), e(self.head_dim))
+                           for _ in range(c.num_hidden_layers)]
         scale = self.head_dim ** -0.5
         self.attn = [Attention(self.num_heads, self.head_dim, scale, self.num_kv_heads) for _ in self.layers]
         for i, a in enumerate(self.attn):
@@ -170,20 +188,15 @@ class Qwen3ForCausalLM:
         assert parts[0] == "model" and parts[1] == "layers", name
         L = self.layers[int(parts[2])]
         leaf = ".".join(parts[3:-1])
-        if leaf == "self_attn.q_proj":
-            L.qkv[:self.q_size].copy_(w.chunk(n, 0)[r])
-        elif leaf == "self_attn.k_proj":
-            L.qkv[self.q_size:self.q_size + self.kv_size].copy_(w.chunk(n, 0)[r])
-        elif leaf == "self_attn.v_proj":
-            L.qkv[self.q_size + self.kv_size:].copy_(w.chunk(n, 0)[r])
-        elif leaf == "self_attn.o_proj":
-            L.o.copy_(w.chunk(n, 1)[r])
-        elif leaf == "mlp.gate_proj":
-            L.gate_up[:self.inter].copy_(w.chunk(n, 0)[r])
-        elif leaf == "mlp.up_proj":
-            L.gate_up[self.inter:].copy_(w.chunk(n, 0)[r])
-        elif leaf == "mlp.down_proj":
-            L.down.copy_(w.chunk(n, 1)[r])
+        if leaf in fp8fmt.PROJECTIONS:
+            scale = parts[-1] == "weight_scale_inv"
+            if scale and not self.fp8:
+                raise NotImplementedError(f"{name}: block-FP8 scales in a checkpoint whose config.json has no fp8 quantization_config")
+            if not scale and self.fp8 != (w.dtype == torch.float8_e4m3fn):
+                raise NotImplementedError(f"{name} is {w.dtype}, but the checkpoint's config.json says "
+                                          f"{'block-FP8 (e4m3)' if self.fp8 else 'unquantized'} projections")
+            dst, dim = self._projection_slot(L, leaf, scale)
+            dst.copy_(w.chunk(n, dim)[r])        # scales: column-parallel rows / row-parallel columns, whole 128-blocks
         elif leaf == "input_layernorm":
             L.ln1.copy_(w)
         elif leaf == "post_attention_layernorm":
@@ -195,11 +208,42 @@ class Qwen3ForCausalLM:
         else:
             raise KeyError(f"unexpected checkpoint tensor {name}")
 
+    def _projection_slot(self, L: LayerWeights, leaf: str, scale: bool):
+        """(destination, tensor-parallel split dim) of a projection weight, or of its block scales (one row / column per
+        128 weight rows / columns): q/k/v pack into qkv, gate/up into gate_up (linear.py:65-70,87-93,114-128,142-150)."""
+        b = fp8fmt.BLOCK if scale else 1
+        q, kv, inter = self.q_size // b, self.kv_size // b, self.inter // b
+        qkv, o, gu, down = (L.qkv_s, L.o_s, L.gate_up_s, L.down_s) if scale else (L.qkv, L.o, L.gate_up, L.down)
+        return {"self_attn.q_proj": (qkv[:q], 0), "self_attn.k_proj": (qkv[q:q + kv], 0), "self_attn.v_proj": (qkv[q + kv:], 0),
+                "self_attn.o_proj": (o, 1), "mlp.gate_proj": (gu[:inter], 0), "mlp.up_proj": (gu[inter:], 0),
+                "mlp.down_proj": (down, 1)}[leaf]
+
     def modules(self):
         """The attention operators, in layer order (what allocate_kv_cache walks, model_runner.py:116-121)."""
         return iter(self.attn)
 
     # ---- forward -------------------------------------------------------------------------------
+    def _fp8_linear(self, x: torch.Tensor, w: torch.Tensor, s: torch.Tensor, epilogue: int, block_n: int, k_splits: int = 1,
+                    out: torch.Tensor | None = None) -> torch.Tensor:
+        """Block-FP8 projection: per-token e4m3 quantization of x, then the wgmma e4m3 GEMM (csrc/linear_tc.cu)."""
+        pdl = bool(self.tc_cfg[6])
+        xq, xs = ops.quant_fp8(x)
+        return ops.linear_fp8(xq, xs, w, s, epilogue, block_n, k_splits, pdl=pdl, out=out)
+
+    def _row_linear_fp8(self, x: torch.Tensor, w: torch.Tensor, s: torch.Tensor):
+        """_row_linear on block-FP8 weights: split-K fp32 partials for decode-size batches on one GPU, bf16 into the
+        peer-mapped buffer under tensor parallelism, a bf16 output otherwise (prefill)."""
+        t, peer = x.shape[0], self.peer
+        if self.tp_size == 1 and t <= 128:
+            kb = x.shape[1] // fp8fmt.BLOCK
+            splits = next(d for d in range(min(8, kb), 0, -1) if kb % d == 0)
+            return self._fp8_linear(x, w, s, ops.EPI_PARTIAL, 64, splits), "parts"
+        if peer is not None and t <= peer.rows_cap:
+            out = peer.next_out(t)
+            self._fp8_linear(x, w, s, ops.EPI_BF16, 32, out=out)
+            return out, True
+        return self._fp8_linear(x, w, s, ops.EPI_BF16, 64), False
+
     def _row_linear(self, x: torch.Tensor, w: torch.Tensor, tc=None):
         """Row-parallel GEMM (o_proj / down_proj).  Returns (partial, where): where is True when the partial sits in
         the peer-mapped buffer, "parts" when it is the fp32 split-K partials of the wgmma path."""
@@ -360,9 +404,12 @@ class Qwen3ForCausalLM:
                 residual, x = h, ops.rmsnorm(h, L.ln1, eps)
             else:
                 x, residual = self._reduce_add_norm(h, in_peer, residual, L.ln1)
-            qkv = ops.linear(x, L.qkv, ops.EPI_BF16, cfg[0], pdl=bool(cfg[6])) if (tc and self.tc_cols) else F.linear(x, L.qkv)
+            t = x.shape[0]
+            if self.fp8:
+                qkv = self._fp8_linear(x, L.qkv, L.qkv_s, ops.EPI_BF16, 64)
+            else:
+                qkv = ops.linear(x, L.qkv, ops.EPI_BF16, cfg[0], pdl=bool(cfg[6])) if (tc and self.tc_cols) else F.linear(x, L.qkv)
             cached = attn.k_cache.numel() > 0
-            t = qkv.shape[0]
             if cached and not ctx.is_prefill and t <= self.fused_decode_max_batch:
                 # decode: q/k-norm, RoPE, KV append and attention in ONE launch on the raw projection output
                 o = ops.paged_decode_fused(li, qkv, hq, L.q_norm, L.k_norm, self.cos_sin, eps, ctx.block_tables,
@@ -375,13 +422,21 @@ class Qwen3ForCausalLM:
                 v = qkv[:, self.q_size + self.kv_size:].view(t, hkv, d)
                 o = attn(q, k, v, kv_stored=True)
             big = tc and t > 128
-            h, in_peer = self._row_linear(o.reshape(t, self.q_size), L.o, (cfg[2], self.tc_big[0] if big else cfg[3]) if tc else None)
+            if self.fp8:
+                h, in_peer = self._row_linear_fp8(o.reshape(t, self.q_size), L.o, L.o_s)
+            else:
+                h, in_peer = self._row_linear(o.reshape(t, self.q_size), L.o, (cfg[2], self.tc_big[0] if big else cfg[3]) if tc else None)
             x, residual = self._reduce_add_norm(h, in_peer, residual, L.ln2)
-            if (tc and self.tc_cols) or (self.tc_gate_up and not ctx.is_prefill and t <= self.tc_gate_up_max):
+            if self.fp8:
+                act = self._fp8_linear(x, L.gate_up, L.gate_up_s, ops.EPI_SILU, 64)
+            elif (tc and self.tc_cols) or (self.tc_gate_up and not ctx.is_prefill and t <= self.tc_gate_up_max):
                 act = ops.linear(x, L.gate_up, ops.EPI_SILU, cfg[1], pdl=bool(cfg[6]))
             else:
                 act = ops.silu_mul(F.linear(x, L.gate_up))
-            h, in_peer = self._row_linear(act, L.down, (cfg[4], self.tc_big[1] if big else cfg[5]) if tc else None)
+            if self.fp8:
+                h, in_peer = self._row_linear_fp8(act, L.down, L.down_s)
+            else:
+                h, in_peer = self._row_linear(act, L.down, (cfg[4], self.tc_big[1] if big else cfg[5]) if tc else None)
         x, _ = self._reduce_add_norm(h, in_peer, residual, self.norm)
         return x
 

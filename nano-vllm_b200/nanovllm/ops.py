@@ -555,6 +555,45 @@ def linear(x: torch.Tensor, w: torch.Tensor, epilogue: int = EPI_BF16, block_n: 
     return out
 
 
+def quant_fp8(x: torch.Tensor, out: torch.Tensor | None = None, scales: torch.Tensor | None = None):
+    """Dynamic per-token, per-128-column e4m3 quantization of x [rows, k] bf16 -> (q [rows, k] e4m3, scales [rows, k/128] fp32)."""
+    _need(x, torch.bfloat16, "x")
+    assert x.dim() == 2 and x.stride(1) == 1
+    rows, k = x.shape
+    if out is None:
+        out = torch.empty(rows, k, dtype=torch.float8_e4m3fn, device=x.device)
+    if scales is None:
+        scales = torch.empty(rows, k // 128, dtype=torch.float32, device=x.device)
+    nat.check(nat.load().b200_quant_fp8(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), scales.data_ptr(),
+                                        scales.stride(0), rows, k, _stream()))
+    return out, scales
+
+
+def linear_fp8(xq: torch.Tensor, x_scale: torch.Tensor, w: torch.Tensor, w_scale: torch.Tensor, epilogue: int = EPI_BF16,
+               block_n: int = 64, k_splits: int = 1, pdl: bool = False, out: torch.Tensor | None = None,
+               shallow: bool = False, cluster: int = 1, stages: int = 0) -> torch.Tensor:
+    """``linear`` on block-scaled e4m3 operands: xq [rows, k] with x_scale [rows, k/128] (``quant_fp8``), w [n, k] with
+    w_scale [n/128, k/128].  Same epilogues and flags as ``linear``."""
+    _need(xq, torch.float8_e4m3fn, "xq"); _need(w, torch.float8_e4m3fn, "w")
+    _need(x_scale, torch.float32, "x_scale"); _need(w_scale, torch.float32, "w_scale")
+    assert xq.dim() == 2 and w.dim() == 2 and xq.stride(1) == 1 and w.is_contiguous() and xq.shape[1] == w.shape[1]
+    rows, k = xq.shape
+    assert w_scale.is_contiguous() and w_scale.shape == (w.shape[0] // 128, k // 128)
+    assert x_scale.stride(1) == 1 and x_scale.shape == (rows, k // 128)
+    n_out = w.shape[0] // 2 if epilogue == EPI_SILU else w.shape[0]
+    if out is None:
+        if epilogue == EPI_PARTIAL:
+            out = torch.empty(k_splits, rows, n_out, dtype=torch.float32, device=xq.device)
+        else:
+            out = torch.empty(rows, n_out, dtype=torch.bfloat16, device=xq.device)
+    nat.check(nat.load().b200_linear_fp8(xq.data_ptr(), xq.stride(0), x_scale.data_ptr(), x_scale.stride(0), w.data_ptr(),
+                                         w_scale.data_ptr(), out.data_ptr(), out.stride(-2), rows, n_out, k, epilogue, block_n,
+                                         k_splits,
+                                         int(pdl) | (2 if shallow else 0) | ({1: 0, 2: 1, 4: 2}[cluster] << 2) | ((stages & 15) << 4),
+                                         _stream()))
+    return out
+
+
 def add_rmsnorm_partials(partials: torch.Tensor, residual: torch.Tensor, weight: torch.Tensor, eps: float,
                          pdl: bool = False, out: torch.Tensor | None = None):
     """residual <- bf16(bf16(sum_s partials[s]) + residual); returns (rmsnorm(residual) * weight, residual)."""

@@ -34,8 +34,12 @@ def _random_fill(model, seed: int, init_std: float = 0.02) -> int:
     offline).  On a CUDA model every tensor is drawn ON THE DEVICE from a generator keyed by (seed, parameter name) at
     its FULL shape and handed to ``load_hf_tensor``, which slices this rank's shard -- so all tensor-parallel ranks hold
     shards of one well-defined model without 64 GB of host memory or a broadcast.  On a CPU model the values are
-    ``synthetic.random_weights`` (what the tests compare against)."""
-    from .synthetic import random_weights, weight_shapes
+    ``synthetic.random_weights`` (what the tests compare against).
+
+    A block-FP8 model (its config's quantization_config) gets the same bf16 draws, each projection block-quantized
+    (``fp8.quantize_weight``) into its e4m3 weight and ``weight_scale_inv``: the quantized version of the bf16 model of the
+    same seed."""
+    from .synthetic import quantize_checkpoint, random_weights, weight_shapes
     c = model.cfg
     dims = dict(hidden_size=c.hidden_size, num_hidden_layers=c.num_hidden_layers,
                 num_attention_heads=c.num_attention_heads, num_key_value_heads=c.num_key_value_heads,
@@ -43,16 +47,25 @@ def _random_fill(model, seed: int, init_std: float = 0.02) -> int:
                 tie_word_embeddings=model.tie)
     if model.device.type != "cuda":
         ws = random_weights(dims, seed)
+        if model.fp8:
+            ws = quantize_checkpoint(ws)
         for name, w in ws.items():
             model.load_hf_tensor(name, w)
         return len(ws)
     import zlib
+    from .fp8 import quantize_weight
+    from .synthetic import is_projection
     gen = torch.Generator(device=model.device)
     shapes = weight_shapes(dims)
     for name, shape in shapes.items():
         gen.manual_seed((seed << 32) ^ zlib.crc32(name.encode()))
         w = torch.randn(shape, generator=gen, device=model.device, dtype=torch.float32)
         w = (1.0 + 0.1 * w) if len(shape) == 1 else init_std * w
-        model.load_hf_tensor(name, w.to(torch.bfloat16))
+        w = w.to(torch.bfloat16)
+        if model.fp8 and is_projection(name):
+            q, s = quantize_weight(w)
+            model.load_hf_tensor(name + "_scale_inv", s)
+            w = q
+        model.load_hf_tensor(name, w)
         del w
     return len(shapes)

@@ -71,6 +71,26 @@ def random_weights(dims: dict, seed: int = 0, init_std: float = 0.02) -> dict[st
     return out
 
 
+def is_projection(name: str) -> bool:
+    """A q/k/v/o/gate/up/down weight: what a block-FP8 checkpoint stores as e4m3 with a weight_scale_inv."""
+    from .fp8 import PROJECTIONS
+    return name.endswith(".weight") and name.split(".")[-2] in {p.split(".")[-1] for p in PROJECTIONS}
+
+
+def quantize_checkpoint(weights: dict[str, torch.Tensor], scale_dtype=torch.float32) -> dict[str, torch.Tensor]:
+    """A bf16 checkpoint in Qwen's block-FP8 layout: every projection becomes e4m3 ``<name>`` plus ``<name>_scale_inv``
+    (fp8.quantize_weight); everything else is kept as it is."""
+    from .fp8 import quantize_weight
+    out = {}
+    for name, w in weights.items():
+        if is_projection(name):
+            q, s = quantize_weight(w)
+            out[name], out[name + "_scale_inv"] = q, s.to(scale_dtype)
+        else:
+            out[name] = w
+    return out
+
+
 def write_tokenizer(path: str, vocab_size: int, eos_id: int = 1) -> None:
     vocab = {f"t{i}": i for i in range(vocab_size)}
     vocab[f"t{eos_id}"] = eos_id
@@ -86,23 +106,32 @@ def write_tokenizer(path: str, vocab_size: int, eos_id: int = 1) -> None:
 
 
 def make_model_dir(path: str, preset: str | dict = "qwen3-0.6b", seed: int = 0, init_std: float = 0.02,
-                   weights: bool = True, tokenizer: bool = True) -> str:
-    """Create (idempotently) a loadable model directory; returns ``path``."""
+                   weights: bool = True, tokenizer: bool = True, fp8: bool = False) -> str:
+    """Create (idempotently) a loadable model directory; returns ``path``.  ``fp8``: a block-FP8 checkpoint in Qwen's
+    format (its quantization_config in config.json; the weights, if written, are the bf16 draws of the same seed
+    block-quantized, see ``quantize_checkpoint``)."""
     dims = dict(PRESETS[preset]) if isinstance(preset, str) else dict(preset)
     os.makedirs(path, exist_ok=True)
     stamp = os.path.join(path, ".synthetic.json")
     want = dict(dims=dims, seed=seed, init_std=init_std, weights=weights, tokenizer=tokenizer, v=2)
+    if fp8:
+        want["fp8"] = True
     if os.path.exists(stamp):
         with open(stamp) as f:
             if json.load(f) == want:
                 return path
+    cfg = hf_config_dict(dims)
+    if fp8:
+        from .fp8 import quantization_config_dict
+        cfg["quantization_config"] = quantization_config_dict()
     with open(os.path.join(path, "config.json"), "w") as f:
-        json.dump(hf_config_dict(dims), f, indent=1)
+        json.dump(cfg, f, indent=1)
     if tokenizer:
         write_tokenizer(path, dims["vocab_size"])
     if weights:
         from safetensors.torch import save_file
-        save_file(random_weights(dims, seed, init_std), os.path.join(path, "model.safetensors"))
+        ws = random_weights(dims, seed, init_std)
+        save_file(quantize_checkpoint(ws) if fp8 else ws, os.path.join(path, "model.safetensors"))
     with open(stamp, "w") as f:
         json.dump(want, f)
     return path
