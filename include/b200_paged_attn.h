@@ -384,6 +384,40 @@ int b200_linear_fp8(const void* x, int64_t x_stride0, const float* x_scale, int6
                     const float* w_scale, void* out, int64_t out_stride0, int rows, int n_out, int k, int epilogue,
                     int block_n, int k_splits, int flags, void* stream);
 
+/* ---- mixture-of-experts MLP of Qwen3 MoE checkpoints (Qwen3MoeSparseMoeBlock; csrc/moe.cu, DESIGN.md 3.7) -----------
+ *
+ * T tokens, E experts (E <= 256), top_k experts per token (top_k <= 16, top_k <= E); an entry is a (token t, rank j)
+ * pair, entry index t * top_k + j.  Launch grids depend on T only, so a captured step serves every routing.
+ * b200_moe_route: logits [T, E] bf16 (row stride logits_stride0 >= E) -> per token the top_k experts by fp32 softmax
+ *   probability (expf; descending, ties to the lower expert id) in topk_ids [T, top_k] int32 and their fp32 probabilities in
+ *   topk_weights [T, top_k], divided by their fp32 sum in rank order when norm_topk is non-zero.
+ * b200_moe_max_tiles: rows of the tile table b200_moe_align may write for `entries` entries (ceil(entries / 128) +
+ *   min(E, entries)), -1 on bad arguments.
+ * b200_moe_align: from topk_ids [entries] -> perm [entries] int32, the row of every entry in the permuted buffer (one
+ *   contiguous segment per expert, experts in id order, rows of a segment in no particular order), and the tile table
+ *   tiles [1 + max_tiles] x int4 (16-byte aligned): {n_tiles, rows, 0, 0}, then per tile {expert, first row, end row, 0}
+ *   of at most 128 rows.  B200_EWORKSPACE when max_tiles < b200_moe_max_tiles(entries, E).
+ * b200_moe_gather: x_perm[perm[t top_k + j]] = x[t]; x [T, hidden] bf16 (row stride x_stride0), x_perm [T top_k, hidden]
+ *   contiguous; hidden % 8 == 0.
+ * b200_moe_linear: the grouped wgmma GEMM of b200_linear: out[r] = x[r] w_e^T for every row r of every tile of expert e,
+ *   x [rows, k] bf16 contiguous (the permuted buffer, rows = T top_k), w [num_experts, w_rows, k] bf16 contiguous,
+ *   out [rows, n_out] (row stride out_stride0); epilogue 0 (w_rows = n_out) or 1 (w_rows = 2 n_out: each expert's gate
+ *   rows then its up rows, out = SiluAndMul), block_n as b200_linear; max_tiles as given to b200_moe_align; flags: bit 0
+ *   PDL, bits 4-7 ring depth.
+ * b200_moe_combine: out[t] = bf16(sum_j topk_weights[t, j] y[perm[t top_k + j]]), an fp32 fma chain in rank order j;
+ *   y [T top_k, hidden] contiguous, out [T, hidden] (row stride out_stride0). */
+int b200_moe_max_tiles(int entries, int num_experts);
+int b200_moe_route(const void* logits, int64_t logits_stride0, int tokens, int num_experts, int top_k, int norm_topk,
+                   int32_t* topk_ids, float* topk_weights, void* stream);
+int b200_moe_align(const int32_t* topk_ids, int entries, int num_experts, int32_t* perm, int32_t* tiles, int max_tiles,
+                   void* stream);
+int b200_moe_gather(const void* x, int64_t x_stride0, int tokens, int hidden, int top_k, const int32_t* perm, void* x_perm,
+                    void* stream);
+int b200_moe_linear(const void* x, const void* w, void* out, int64_t out_stride0, int rows, int num_experts, int n_out, int k,
+                    const int32_t* tiles, int max_tiles, int epilogue, int block_n, int flags, void* stream);
+int b200_moe_combine(const void* y, const int32_t* perm, const float* topk_weights, int tokens, int hidden, int top_k,
+                     void* out, int64_t out_stride0, void* stream);
+
 /* (opt-in) ParallelLMHead.forward + Sampler.forward in one pass (layers/embed_head.py:56-66, layers/sampler.py:7-12):
  * logits = bf16(hidden lm_head^T) are produced tile by tile in registers, scored exactly as b200_sample scores
  * them (same RNG keyed by (seed, step, row, vocabulary id); temperature 0 = greedy, lowest index on ties) and

@@ -40,6 +40,11 @@ constexpr uint32_t X_TILE = LM * 128;     // 16 KB
 constexpr uint32_t X_HALF = 64 * 128;     // 8 KB: rows [64, 128) of the x tile
 
 enum { EPI_BF16 = 0, EPI_SILU = 1, EPI_PARTIAL = 2, EPI_SAMPLE = 3 };
+// Grouped (mixture-of-experts) mode, or-ed into EPI_BF16 / EPI_SILU (b200_moe_linear): W stacks the experts' weights,
+// [E * w_rows, k], and x holds the tokens' rows permuted into one contiguous segment per expert.  blockIdx.y names a tile
+// of the device tile table (expert, first row, end row); CTAs past the table's tile count exit, so one grid serves every
+// routing and a captured step stays valid whatever the router picks.
+constexpr int EPI_GROUPED = 4;
 
 // DEEP: as many ring slots as one CTA per SM allows (all of a short K in flight).  !DEEP: 4 slots for block_n <= 64, so
 // that two CTAs fit an SM and a dependent kernel launched early (PDL) finds room to prefetch its weights.
@@ -62,11 +67,15 @@ struct LinParams {
     int stages;               // ring slots of this launch (2 .. Cfg::STAGES)
     // EPI_SAMPLE (fused LM head + sampling): nothing of size [rows, vocab] is ever written
     int n_valid;                          // columns of this vocabulary shard (the last column block may be ragged)
+    int expert_rows;                      // EPI_GROUPED: W rows of one expert (n_out, 2 * n_out for EPI_SILU)
     const float* temperatures;            // [rows] or null (greedy)
     int64_t index_offset;                 // first vocabulary id of the shard
     uint64_t seed, step;
     const int64_t* step_dev;              // optional device-side addend to step (CUDA-graph replays)
-    unsigned long long* keys;             // [rows] running maximum of packed (score, token) keys; zero = empty
+    union {
+        unsigned long long* keys;         // [rows] running maximum of packed (score, token) keys; zero = empty
+        const int4* tiles;                // EPI_GROUPED: {n_tiles, ...} then n_tiles x {expert, first row, end row, 0}
+    };
 };
 
 __device__ __forceinline__ void tma_load_2d_hint(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, uint64_t policy) {
@@ -120,10 +129,12 @@ template <int BN, int EPI, bool DEEP, int CL, bool FP8>
 __global__ void __launch_bounds__(L_THREADS, 1)
 linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, const LinParams p, const Fp8Scales fs) {
     using C = Cfg<BN, DEEP>;
+    constexpr bool GROUPED = (EPI & EPI_GROUPED) != 0;
+    constexpr int EP = EPI & ~EPI_GROUPED;                   // the epilogue
     constexpr uint16_t CL_MASK = (uint16_t)((1u << CL) - 1);
     constexpr int X_ROWS = LM / CL;                            // rows of x this CTA fetches (and multicasts when CL > 1)
     const int S = p.stages;
-    constexpr int BOUT = EPI == EPI_SILU ? BN / 2 : BN;       // output columns of this CTA
+    constexpr int BOUT = EP == EPI_SILU ? BN / 2 : BN;        // output columns of this CTA
     extern __shared__ __align__(1024) uint8_t smem_raw[];     // 128-byte swizzle atoms need 1024-byte alignment
     const uint32_t base = smem_u32(smem_raw);
     if (base & 1023u) __trap();
@@ -137,10 +148,21 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
     const int tid = threadIdx.x;
     const int warp = tid >> 5;
     const int lane = tid & 31;
-    const int m0 = blockIdx.y * LM;
+    int m0 = blockIdx.y * LM;
+    int row_end = p.rows;                                      // rows [m0, row_end) of x are this CTA's to store
+    int w_row0 = 0;                                            // first W row of this CTA's expert
+    if constexpr (GROUPED) {
+        // the tile table is the previous kernel's output, so grouped CTAs cannot prefetch weights before the wait
+        asm volatile("griddepcontrol.wait;" ::: "memory");
+        if ((int)blockIdx.y >= p.tiles[0].x) return;
+        const int4 t = p.tiles[1 + blockIdx.y];
+        w_row0 = t.x * p.expert_rows;
+        m0 = t.y;
+        row_end = t.z;
+    }
     const int kt0 = blockIdx.z * p.k_tiles;
     const int nk = p.k_tiles;
-    const bool two_halves = p.rows - m0 > 64;                 // rows [64, 128) of this CTA exist
+    const bool two_halves = row_end - m0 > 64;                 // rows [64, 128) of this CTA exist
 
     const uint32_t crank = CL > 1 ? cluster_ctarank() : 0;
     if (tid == 0) {
@@ -158,11 +180,11 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
             const uint64_t pol = l2_policy_evict_first();
             auto load_w = [&](int slot, int kt) {
                 const uint32_t dst = base + slot * C::STAGE + X_TILE;
-                if constexpr (EPI == EPI_SILU) {
-                    tma_load_2d_hint(dst, &tm_w, bars + slot * 8, kt * LK, blockIdx.x * BOUT, pol);
-                    tma_load_2d_hint(dst + BOUT * 128, &tm_w, bars + slot * 8, kt * LK, p.up_row0 + blockIdx.x * BOUT, pol);
+                if constexpr (EP == EPI_SILU) {
+                    tma_load_2d_hint(dst, &tm_w, bars + slot * 8, kt * LK, w_row0 + blockIdx.x * BOUT, pol);
+                    tma_load_2d_hint(dst + BOUT * 128, &tm_w, bars + slot * 8, kt * LK, w_row0 + p.up_row0 + blockIdx.x * BOUT, pol);
                 } else {
-                    tma_load_2d_hint(dst, &tm_w, bars + slot * 8, kt * LK, blockIdx.x * BN, pol);
+                    tma_load_2d_hint(dst, &tm_w, bars + slot * 8, kt * LK, w_row0 + blockIdx.x * BN, pol);
                 }
             };
             auto load_x = [&](int slot, int kt) {
@@ -202,7 +224,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
                 asm volatile("griddepcontrol.wait;" ::: "memory");   // x_scale is the previous kernel's output
                 float part[2][BN / 2];
                 const int g = lane >> 2;
-                const int wrow = EPI == EPI_SILU ? blockIdx.x * BOUT : blockIdx.x * BN;
+                const int wrow = EP == EPI_SILU ? blockIdx.x * BOUT : blockIdx.x * BN;
                 const float* ws_gate = fs.w_scale + (int64_t)(wrow / 128) * fs.ws_cols;
                 const float* ws_up = fs.w_scale + (int64_t)((p.up_row0 + wrow) / 128) * fs.ws_cols;
                 // Scales are read SPF blocks ahead into registers (slot j of the unrolled loop holds block i0 + j), so that
@@ -213,13 +235,13 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
                     if (i >= nk) return;
                     const int kb = kt0 + i;
                     wg = ws_gate[kb];
-                    wu = EPI == EPI_SILU ? ws_up[kb] : wg;
+                    wu = EP == EPI_SILU ? ws_up[kb] : wg;
 #pragma unroll
                     for (int h = 0; h < 2; ++h)
 #pragma unroll
                         for (int r = 0; r < 2; ++r) {
                             const int row = m0 + 64 * h + 16 * warp + g + 8 * r;      // rows past `rows` are never stored
-                            x[h][r] = row < p.rows ? fs.x_scale[(int64_t)row * fs.xs_stride + kb] : 0.f;
+                            x[h][r] = row < row_end ? fs.x_scale[(int64_t)row * fs.xs_stride + kb] : 0.f;
                         }
                 };
 #pragma unroll
@@ -259,7 +281,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
                             for (int c = 0; c < BN / 8; ++c)
 #pragma unroll
                                 for (int r = 0; r < 2; ++r) {
-                                    const float sc = (EPI == EPI_SILU && c >= BOUT / 8) ? su[h][r] : sg[h][r];
+                                    const float sc = (EP == EPI_SILU && c >= BOUT / 8) ? su[h][r] : sg[h][r];
                                     acc[h][4 * c + 2 * r] = fmaf(part[h][4 * c + 2 * r], sc, acc[h][4 * c + 2 * r]);
                                     acc[h][4 * c + 2 * r + 1] = fmaf(part[h][4 * c + 2 * r + 1], sc, acc[h][4 * c + 2 * r + 1]);
                                 }
@@ -299,7 +321,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
 #pragma unroll
             for (int r = 0; r < 2; ++r) {
                 const int row = m0 + 64 * h + 16 * warp + g + 8 * r;
-                if constexpr (EPI == EPI_SAMPLE) {
+                if constexpr (EP == EPI_SAMPLE) {
                     // LM head + Sampler.forward in one pass (layers/embed_head.py:56-66, layers/sampler.py:7-12): this thread
                     // holds BN/4 logits of its row; they are rounded to bf16 (the reference's logits are the bf16 output of
                     // F.linear), scored (greedy: the logit; otherwise the exponential race) and only the best (score, token)
@@ -322,8 +344,8 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
                     key = max(key, __shfl_xor_sync(0xffffffffu, key, 1));
                     key = max(key, __shfl_xor_sync(0xffffffffu, key, 2));
                     if (qd == 0 && key != 0ull) atomicMax(p.keys + row, key);
-                } else if (row < p.rows) {
-                    if constexpr (EPI == EPI_PARTIAL) {
+                } else if (row < row_end) {
+                    if constexpr (EP == EPI_PARTIAL) {
                         float* dst = static_cast<float*>(p.out) + ((int64_t)blockIdx.z * p.rows + row) * p.out_stride + blockIdx.x * BN + 2 * qd;
 #pragma unroll
                         for (int c = 0; c < BN / 8; ++c) *reinterpret_cast<float2*>(dst + 8 * c) = make_float2(acc[h][4 * c + 2 * r], acc[h][4 * c + 2 * r + 1]);
@@ -334,7 +356,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant
                             float y[2];
 #pragma unroll
                             for (int e = 0; e < 2; ++e) {
-                                if constexpr (EPI == EPI_SILU) {
+                                if constexpr (EP == EPI_SILU) {
                                     // the reference rounds the projection to bf16 before SiluAndMul sees it (F.linear output)
                                     const float gt = round_bf16(acc[h][4 * c + 2 * r + e]), up = round_bf16(acc[h][4 * (c + BOUT / 8) + 2 * r + e]);
                                     y[e] = __fmul_rn(gt / (1.0f + expf(-gt)), up);
@@ -517,7 +539,7 @@ int launch_linear(const CUtensorMap& tx, const CUtensorMap& tw, LinParams prm, c
 template <int EPI, bool DEEP, int CL, bool FP8>
 int dispatch_bn(int bn, const CUtensorMap& tx, const CUtensorMap& tw, const LinParams& prm, const Fp8Scales& fs, dim3 grid, bool pdl, cudaStream_t stream) {
     switch (bn) {
-        case 16: if constexpr (EPI == EPI_SILU) return B200_EUNSUPPORTED; else return launch_linear<16, EPI, DEEP, CL, FP8>(tx, tw, prm, fs, grid, pdl, stream);
+        case 16: if constexpr ((EPI & ~EPI_GROUPED) == EPI_SILU) return B200_EUNSUPPORTED; else return launch_linear<16, EPI, DEEP, CL, FP8>(tx, tw, prm, fs, grid, pdl, stream);
         case 32: return launch_linear<32, EPI, DEEP, CL, FP8>(tx, tw, prm, fs, grid, pdl, stream);
         case 64: return launch_linear<64, EPI, DEEP, CL, FP8>(tx, tw, prm, fs, grid, pdl, stream);
         case 128: if constexpr (FP8) return B200_EUNSUPPORTED; else return launch_linear<128, EPI, DEEP, CL, FP8>(tx, tw, prm, fs, grid, pdl, stream);
@@ -697,6 +719,43 @@ extern "C" int b200_linear_fp8(const void* x, int64_t x_stride0, const float* x_
     if (epilogue == EPI_BF16) rc = dispatch_depth<EPI_BF16, true>(deep, cluster, block_n, tx, tw, prm, grid, pdl, st, fs);
     else if (epilogue == EPI_SILU) rc = dispatch_depth<EPI_SILU, true>(deep, cluster, block_n, tx, tw, prm, grid, pdl, st, fs);
     else rc = dispatch_depth<EPI_PARTIAL, true>(deep, cluster, block_n, tx, tw, prm, grid, pdl, st, fs);
+    if (rc != B200_OK) return rc;
+    return b200_launch_status(nullptr);
+}
+
+extern "C" int b200_moe_linear(const void* x, const void* w, void* out, int64_t out_stride0, int rows, int num_experts, int n_out,
+                               int k, const int32_t* tiles, int max_tiles, int epilogue, int block_n, int flags, void* stream) {
+    if (!x || !w || !out || !tiles || rows < 0 || num_experts <= 0 || n_out <= 0 || k <= 0 || max_tiles < 0) return B200_EINVAL;
+    if (((uintptr_t)x & 15) || ((uintptr_t)w & 15) || ((uintptr_t)out & 15) || ((uintptr_t)tiles & 15) || (out_stride0 % 8))
+        return B200_EINVAL;
+    if (epilogue != EPI_BF16 && epilogue != EPI_SILU) return B200_EINVAL;
+    if (out_stride0 < n_out) return B200_EINVAL;
+    if (k % LK) return B200_EUNSUPPORTED;
+    if (block_n != 32 && block_n != 64 && block_n != 128 && !(block_n == 16 && epilogue == EPI_BF16)) return B200_EUNSUPPORTED;
+    const int bout = epilogue == EPI_SILU ? block_n / 2 : block_n;
+    if (n_out % bout) return B200_EUNSUPPORTED;
+    if (max_tiles > 65535) return B200_EUNSUPPORTED;
+    if (rows == 0 || max_tiles == 0) return B200_OK;
+    const int expert_rows = epilogue == EPI_SILU ? 2 * n_out : n_out;
+    if ((int64_t)num_experts * expert_rows > 0x7fffffff) return B200_EUNSUPPORTED;
+    CUtensorMap tx, tw;
+    if (!cached_map(&tx, x, (uint64_t)k, (uint64_t)rows, (uint64_t)k, LM)) return B200_EUNSUPPORTED;
+    if (!cached_map(&tw, w, (uint64_t)k, (uint64_t)num_experts * expert_rows, (uint64_t)k, (uint32_t)bout)) return B200_EUNSUPPORTED;
+    LinParams prm = {};
+    prm.out = out;
+    prm.out_stride = out_stride0;
+    prm.rows = rows;
+    prm.up_row0 = n_out;
+    prm.k_tiles = k / LK;
+    prm.stages = (flags >> 4) & 15;
+    prm.expert_rows = expert_rows;
+    prm.tiles = reinterpret_cast<const int4*>(tiles);
+    const dim3 grid(n_out / bout, max_tiles, 1);
+    const bool pdl = (flags & 1) != 0;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int rc;
+    if (epilogue == EPI_BF16) rc = dispatch_bn<EPI_GROUPED | EPI_BF16, true, 1, false>(block_n, tx, tw, prm, Fp8Scales{}, grid, pdl, st);
+    else rc = dispatch_bn<EPI_GROUPED | EPI_SILU, true, 1, false>(block_n, tx, tw, prm, Fp8Scales{}, grid, pdl, st);
     if (rc != B200_OK) return rc;
     return b200_launch_status(nullptr);
 }

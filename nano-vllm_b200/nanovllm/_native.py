@@ -56,6 +56,13 @@ SIGNATURES = {
     "b200_quant_fp8": (_i, [_vp, _i64, _vp, _i64, _vp, _i64, _i, _i, _vp]),
     "b200_linear_fp8": (_i, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "b200_add_rmsnorm_partials": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _f, _i, _vp]),
+    # mixture-of-experts MLP (csrc/moe.cu and the grouped mode of csrc/linear_tc.cu)
+    "b200_moe_max_tiles": (_i, [_i, _i]),
+    "b200_moe_route": (_i, [_vp, _i64, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "b200_moe_align": (_i, [_vp, _i, _i, _vp, _vp, _i, _vp]),
+    "b200_moe_gather": (_i, [_vp, _i64, _i, _i, _i, _vp, _vp, _vp]),
+    "b200_moe_linear": (_i, [_vp, _vp, _vp, _i64, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp]),
+    "b200_moe_combine": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _i64, _vp]),
     "b200_lm_head_sample": (_i, [_vp, _i64, _vp, _i, _i, _i, _vp, _i64, _u64, _u64, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     "b200_layer_tail_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "b200_layer_tail": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _vp, _sz, _i, _i, _i, _i, _f, _i, _i, _vp]),

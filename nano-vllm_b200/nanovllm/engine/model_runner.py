@@ -32,7 +32,7 @@ from .. import _native as nat
 from .. import ops
 from ..config import KV_CACHE_DTYPES, Config
 from ..layers.attention import KVGroup, kv_group_arrays, plan_kv_groups
-from ..models.qwen3 import Qwen3ForCausalLM
+from ..models.qwen3_moe import model_class
 from ..utils.context import reset_context, set_context
 from ..utils.loader import load_model
 from .sequence import Sequence, SequenceStatus
@@ -122,7 +122,7 @@ class ModelRunner:
             sample_seed = int(t.item())
         self.sample_seed = sample_seed
 
-        self.model = Qwen3ForCausalLM(hf, rank, self.world_size, self.device, max_position=hf.max_position_embeddings)
+        self.model = model_class(hf)(hf, rank, self.world_size, self.device, max_position=hf.max_position_embeddings)
         load_model(self.model, config.model, allow_random=bool(os.environ.get("NANOVLLM_ALLOW_RANDOM_INIT")))
         self.vocab_offset = rank * self.model.vocab_shard
         if self.world_size > 1:

@@ -49,6 +49,9 @@ class LayerWeights:
     o_s: torch.Tensor | None = None
     gate_up_s: torch.Tensor | None = None
     down_s: torch.Tensor | None = None
+    # mixture-of-experts layers (models/qwen3_moe.py): the router [E, hidden]; gate_up / down are then [E, 2 * I / tp, hidden]
+    # and [E, hidden, I / tp]
+    gate: torch.Tensor | None = None
 
 
 class Qwen3ForCausalLM:
@@ -67,10 +70,10 @@ class Qwen3ForCausalLM:
         self.hidden = c.hidden_size
         self.head_dim = getattr(c, "head_dim", None) or c.hidden_size // c.num_attention_heads
         assert c.num_attention_heads % tp_size == 0 and c.num_key_value_heads % tp_size == 0
-        assert c.vocab_size % tp_size == 0 and c.intermediate_size % tp_size == 0
+        assert c.vocab_size % tp_size == 0 and self._intermediate_size(c) % tp_size == 0
         self.num_heads = c.num_attention_heads // tp_size
         self.num_kv_heads = c.num_key_value_heads // tp_size
-        self.inter = c.intermediate_size // tp_size
+        self.inter = self._intermediate_size(c) // tp_size
         self.vocab_shard = c.vocab_size // tp_size
         self.eps = c.rms_norm_eps
         self.q_size = self.num_heads * self.head_dim
@@ -156,8 +159,7 @@ class Qwen3ForCausalLM:
         self.lm_head = (self.embed[tp_rank * self.vocab_shard:(tp_rank + 1) * self.vocab_shard]
                         if self.tie else e(self.vocab_shard, self.hidden))
         self.norm = e(self.hidden)
-        proj = [(self.q_size + 2 * self.kv_size, self.hidden), (self.hidden, self.q_size), (2 * self.inter, self.hidden),
-                (self.hidden, self.inter)]
+        proj = [(self.q_size + 2 * self.kv_size, self.hidden), (self.hidden, self.q_size), *self._mlp_shapes()]
         if self.fp8:
             q8 = lambda n, k: torch.empty(n, k, dtype=torch.float8_e4m3fn, device=dev)
             sc = lambda n, k: torch.empty(n // fp8fmt.BLOCK, k // fp8fmt.BLOCK, dtype=torch.float32, device=dev)
@@ -171,6 +173,14 @@ class Qwen3ForCausalLM:
         self.attn = [Attention(self.num_heads, self.head_dim, scale, self.num_kv_heads) for _ in self.layers]
         for i, a in enumerate(self.attn):
             a.layer_id = i
+
+    @staticmethod
+    def _intermediate_size(c) -> int:
+        return c.intermediate_size
+
+    def _mlp_shapes(self) -> list[tuple]:
+        """Shapes of this rank's gate_up and down weights."""
+        return [(2 * self.inter, self.hidden), (self.hidden, self.inter)]
 
     # ---- weights -------------------------------------------------------------------------------
     def load_hf_tensor(self, name: str, w: torch.Tensor) -> None:
@@ -427,18 +437,22 @@ class Qwen3ForCausalLM:
             else:
                 h, in_peer = self._row_linear(o.reshape(t, self.q_size), L.o, (cfg[2], self.tc_big[0] if big else cfg[3]) if tc else None)
             x, residual = self._reduce_add_norm(h, in_peer, residual, L.ln2)
-            if self.fp8:
-                act = self._fp8_linear(x, L.gate_up, L.gate_up_s, ops.EPI_SILU, 64)
-            elif (tc and self.tc_cols) or (self.tc_gate_up and not ctx.is_prefill and t <= self.tc_gate_up_max):
-                act = ops.linear(x, L.gate_up, ops.EPI_SILU, cfg[1], pdl=bool(cfg[6]))
-            else:
-                act = ops.silu_mul(F.linear(x, L.gate_up))
-            if self.fp8:
-                h, in_peer = self._row_linear_fp8(act, L.down, L.down_s)
-            else:
-                h, in_peer = self._row_linear(act, L.down, (cfg[4], self.tc_big[1] if big else cfg[5]) if tc else None)
+            h, in_peer = self._mlp(L, x, ctx, tc, big)
         x, _ = self._reduce_add_norm(h, in_peer, residual, self.norm)
         return x
+
+    def _mlp(self, L: LayerWeights, x: torch.Tensor, ctx, tc: bool, big: bool):
+        """gate_up -> SiluAndMul -> down on the normalised x; returns (partial, where) as _row_linear."""
+        t, cfg = x.shape[0], self.tc_cfg
+        if self.fp8:
+            act = self._fp8_linear(x, L.gate_up, L.gate_up_s, ops.EPI_SILU, 64)
+        elif (tc and self.tc_cols) or (self.tc_gate_up and not ctx.is_prefill and t <= self.tc_gate_up_max):
+            act = ops.linear(x, L.gate_up, ops.EPI_SILU, cfg[1], pdl=bool(cfg[6]))
+        else:
+            act = ops.silu_mul(F.linear(x, L.gate_up))
+        if self.fp8:
+            return self._row_linear_fp8(act, L.down, L.down_s)
+        return self._row_linear(act, L.down, (cfg[4], self.tc_big[1] if big else cfg[5]) if tc else None)
 
     __call__ = forward
 

@@ -630,6 +630,120 @@ def lm_head_sample(hidden: torch.Tensor, lm_head: torch.Tensor, temperatures: to
     return out if out is not None else out_keys
 
 
+# ---- mixture-of-experts MLP (csrc/moe.cu, grouped mode of csrc/linear_tc.cu; DESIGN.md 3.7) ------------------------------
+MOE_MAX_EXPERTS, MOE_MAX_TOPK = 256, 16
+
+
+def moe_route(logits: torch.Tensor, top_k: int, norm_topk: bool, ids: torch.Tensor | None = None,
+              weights: torch.Tensor | None = None) -> tuple[torch.Tensor, torch.Tensor]:
+    """bf16 router logits [T, E] -> (int32 expert ids [T, top_k], fp32 weights [T, top_k]), rank order."""
+    _need(logits, torch.bfloat16, "logits")
+    assert logits.dim() == 2 and logits.stride(1) == 1
+    t, e = logits.shape
+    if ids is None:
+        ids = torch.empty(t, top_k, dtype=torch.int32, device=logits.device)
+    if weights is None:
+        weights = torch.empty(t, top_k, dtype=torch.float32, device=logits.device)
+    _need(ids, torch.int32, "ids"); _need(weights, torch.float32, "weights")
+    assert ids.is_contiguous() and weights.is_contiguous() and ids.shape == (t, top_k) and weights.shape == (t, top_k)
+    nat.check(nat.load().b200_moe_route(logits.data_ptr(), logits.stride(0), t, e, top_k, int(norm_topk), ids.data_ptr(),
+                                        weights.data_ptr(), _stream()))
+    return ids, weights
+
+
+def moe_max_tiles(entries: int, num_experts: int) -> int:
+    n = nat.load().b200_moe_max_tiles(entries, num_experts)
+    if n < 0:
+        nat.check(-1)
+    return n
+
+
+def moe_align(ids: torch.Tensor, num_experts: int, perm: torch.Tensor | None = None,
+              tiles: torch.Tensor | None = None) -> tuple[torch.Tensor, torch.Tensor]:
+    """Expert ids (int32, any shape, entries in row-major order) -> (perm int32 [entries]: each entry's row in the
+    permuted buffer, tiles int32 [1 + max_tiles, 4]: {n_tiles, rows, 0, 0} then {expert, first row, end row, 0})."""
+    _need(ids, torch.int32, "ids")
+    assert ids.is_contiguous()
+    n = ids.numel()
+    max_tiles = moe_max_tiles(n, num_experts)
+    if perm is None:
+        perm = torch.empty(n, dtype=torch.int32, device=ids.device)
+    if tiles is None:
+        tiles = torch.empty(1 + max_tiles, 4, dtype=torch.int32, device=ids.device)
+    _need(perm, torch.int32, "perm"); _need(tiles, torch.int32, "tiles")
+    assert perm.is_contiguous() and perm.numel() >= n and tiles.is_contiguous() and tiles.dim() == 2 and tiles.shape[1] == 4
+    nat.check(nat.load().b200_moe_align(ids.data_ptr(), n, num_experts, perm.data_ptr(), tiles.data_ptr(), tiles.shape[0] - 1,
+                                        _stream()))
+    return perm, tiles
+
+
+def moe_gather(x: torch.Tensor, top_k: int, perm: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
+    """x [T, hidden] bf16 -> x_perm [T * top_k, hidden] with x_perm[perm[t * top_k + j]] = x[t]."""
+    _need(x, torch.bfloat16, "x"); _need(perm, torch.int32, "perm")
+    assert x.dim() == 2 and x.stride(1) == 1 and perm.is_contiguous() and perm.numel() >= x.shape[0] * top_k
+    t, hidden = x.shape
+    if out is None:
+        out = torch.empty(t * top_k, hidden, dtype=x.dtype, device=x.device)
+    _need(out, torch.bfloat16, "out")
+    assert out.is_contiguous() and out.shape == (t * top_k, hidden)
+    nat.check(nat.load().b200_moe_gather(x.data_ptr(), x.stride(0), t, hidden, top_k, perm.data_ptr(), out.data_ptr(), _stream()))
+    return out
+
+
+def moe_linear(x: torch.Tensor, w: torch.Tensor, tiles: torch.Tensor, epilogue: int = EPI_BF16, block_n: int = 64,
+               pdl: bool = False, out: torch.Tensor | None = None, stages: int = 0) -> torch.Tensor:
+    """Grouped GEMM over the permuted rows x [rows, k] and the stacked expert weights w [E, w_rows, k] (``moe_align``'s
+    tiles say which rows belong to which expert).  EPI_SILU: w_rows = 2 n (gate rows, then up rows), returns
+    SiluAndMul [rows, n]; EPI_BF16: returns [rows, w_rows]."""
+    _need(x, torch.bfloat16, "x"); _need(w, torch.bfloat16, "w"); _need(tiles, torch.int32, "tiles")
+    assert x.dim() == 2 and x.is_contiguous() and w.dim() == 3 and w.is_contiguous() and x.shape[1] == w.shape[2]
+    assert tiles.is_contiguous() and tiles.dim() == 2 and tiles.shape[1] == 4
+    if epilogue not in (EPI_BF16, EPI_SILU):
+        nat.check(-1)
+    rows, k = x.shape
+    e = w.shape[0]
+    n_out = w.shape[1] // 2 if epilogue == EPI_SILU else w.shape[1]
+    if out is None:
+        out = torch.empty(rows, n_out, dtype=torch.bfloat16, device=x.device)
+    _need(out, torch.bfloat16, "out")
+    assert out.dim() == 2 and out.stride(1) == 1 and out.shape == (rows, n_out)
+    nat.check(nat.load().b200_moe_linear(x.data_ptr(), w.data_ptr(), out.data_ptr(), out.stride(0), rows, e, n_out, k,
+                                         tiles.data_ptr(), tiles.shape[0] - 1, epilogue, block_n, int(pdl) | ((stages & 15) << 4),
+                                         _stream()))
+    return out
+
+
+def moe_combine(y: torch.Tensor, perm: torch.Tensor, weights: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
+    """y [T * top_k, hidden] (expert outputs in permuted order), weights fp32 [T, top_k] -> bf16 [T, hidden],
+    out[t] = bf16(sum_j weights[t, j] * y[perm[t * top_k + j]]) in rank order."""
+    _need(y, torch.bfloat16, "y"); _need(perm, torch.int32, "perm"); _need(weights, torch.float32, "weights")
+    assert y.is_contiguous() and weights.is_contiguous() and weights.dim() == 2 and perm.is_contiguous()
+    t, top_k = weights.shape
+    hidden = y.shape[1]
+    assert y.shape[0] == t * top_k and perm.numel() >= t * top_k
+    if out is None:
+        out = torch.empty(t, hidden, dtype=torch.bfloat16, device=y.device)
+    _need(out, torch.bfloat16, "out")
+    assert out.dim() == 2 and out.stride(1) == 1 and out.shape == (t, hidden)
+    nat.check(nat.load().b200_moe_combine(y.data_ptr(), perm.data_ptr(), weights.data_ptr(), t, hidden, top_k, out.data_ptr(),
+                                          out.stride(0), _stream()))
+    return out
+
+
+def moe_mlp(x: torch.Tensor, router_logits: torch.Tensor, w_gate_up: torch.Tensor, w_down: torch.Tensor, top_k: int,
+            norm_topk: bool, gate_up_block_n: int = 64, down_block_n: int = 64, pdl: bool = True,
+            out: torch.Tensor | None = None) -> torch.Tensor:
+    """The MoE MLP of Qwen3MoeSparseMoeBlock on the normalised input x [T, hidden] and its bf16 router logits [T, E]:
+    route -> align -> gather -> grouped gate_up + SiluAndMul -> grouped down -> combine (six launches)."""
+    e = w_gate_up.shape[0]
+    ids, weights = moe_route(router_logits, top_k, norm_topk)
+    perm, tiles = moe_align(ids, e)
+    xp = moe_gather(x, top_k, perm)
+    act = moe_linear(xp, w_gate_up, tiles, EPI_SILU, gate_up_block_n, pdl=pdl)
+    y = moe_linear(act, w_down, tiles, EPI_BF16, down_block_n, pdl=pdl)
+    return moe_combine(y, perm, weights, out=out)
+
+
 # ---- the tail of a decoder layer as one persistent kernel (csrc/layer_tail.cu) ---------------------------------------------
 def layer_tail_workspace(max_rows: int, hidden: int, inter: int, max_splits: int, device="cuda") -> torch.Tensor:
     """Zeroed workspace (grid-barrier state, split-K partials, the two intermediate activations)."""

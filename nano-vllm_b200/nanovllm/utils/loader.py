@@ -38,13 +38,17 @@ def _random_fill(model, seed: int, init_std: float = 0.02) -> int:
 
     A block-FP8 model (its config's quantization_config) gets the same bf16 draws, each projection block-quantized
     (``fp8.quantize_weight``) into its e4m3 weight and ``weight_scale_inv``: the quantized version of the bf16 model of the
-    same seed."""
-    from .synthetic import quantize_checkpoint, random_weights, weight_shapes
+    same seed.  A mixture-of-experts model gets the Hub's per-expert names (synthetic.weight_shapes), so its experts are
+    stacked by the same ``load_hf_tensor`` that reads a checkpoint."""
+    from .synthetic import quantize_checkpoint, random_weights, weight_shapes, weight_std
     c = model.cfg
     dims = dict(hidden_size=c.hidden_size, num_hidden_layers=c.num_hidden_layers,
                 num_attention_heads=c.num_attention_heads, num_key_value_heads=c.num_key_value_heads,
                 head_dim=model.head_dim, intermediate_size=c.intermediate_size, vocab_size=c.vocab_size,
                 tie_word_embeddings=model.tie)
+    if getattr(model, "num_experts", 0):
+        dims.update(num_experts=c.num_experts, num_experts_per_tok=c.num_experts_per_tok,
+                    moe_intermediate_size=c.moe_intermediate_size, norm_topk_prob=model.norm_topk)
     if model.device.type != "cuda":
         ws = random_weights(dims, seed)
         if model.fp8:
@@ -60,7 +64,7 @@ def _random_fill(model, seed: int, init_std: float = 0.02) -> int:
     for name, shape in shapes.items():
         gen.manual_seed((seed << 32) ^ zlib.crc32(name.encode()))
         w = torch.randn(shape, generator=gen, device=model.device, dtype=torch.float32)
-        w = (1.0 + 0.1 * w) if len(shape) == 1 else init_std * w
+        w = (1.0 + 0.1 * w) if len(shape) == 1 else weight_std(name, shape, init_std) * w
         w = w.to(torch.bfloat16)
         if model.fp8 and is_projection(name):
             q, s = quantize_weight(w)

@@ -31,13 +31,36 @@ PRESETS = {
                     head_dim=128, intermediate_size=320, vocab_size=1024, tie_word_embeddings=True),
     "tiny-g8": dict(hidden_size=320, num_hidden_layers=2, num_attention_heads=8, num_key_value_heads=1,
                     head_dim=128, intermediate_size=448, vocab_size=3072, tie_word_embeddings=False),
+    # mixture of experts (model_type "qwen3_moe"): intermediate_size is the config's dense-MLP size, unused when every
+    # layer is sparse; the experts' MLPs are moe_intermediate_size wide
+    "qwen3-30b-a3b": dict(hidden_size=2048, num_hidden_layers=48, num_attention_heads=32, num_key_value_heads=4,
+                          head_dim=128, intermediate_size=6144, vocab_size=151936, tie_word_embeddings=False,
+                          num_experts=128, num_experts_per_tok=8, moe_intermediate_size=768, norm_topk_prob=True),
+    "tiny-moe": dict(hidden_size=256, num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=2,
+                     head_dim=128, intermediate_size=512, vocab_size=2048, tie_word_embeddings=True,
+                     num_experts=16, num_experts_per_tok=4, moe_intermediate_size=128, norm_topk_prob=True),
+    # head group 8 (the wide-group decode kernel 30B-A3B runs on), 8 of 32 experts, weights not renormalised
+    "tiny-moe-g8": dict(hidden_size=320, num_hidden_layers=2, num_attention_heads=8, num_key_value_heads=1,
+                        head_dim=128, intermediate_size=448, vocab_size=3072, tie_word_embeddings=False,
+                        num_experts=32, num_experts_per_tok=8, moe_intermediate_size=192, norm_topk_prob=False),
 }
+# Router weights are drawn with std ROUTER_LOGIT_STD / sqrt(hidden), so that router logits have a spread of about
+# ROUTER_LOGIT_STD: with the projections' 0.02 the logits of a small model would all sit within a few bf16 ulps of each
+# other and the routing would be decided by rounding noise.
+ROUTER_LOGIT_STD = 2.0
+
+
+def is_moe(dims: dict) -> bool:
+    return bool(dims.get("num_experts"))
 
 
 def hf_config_dict(dims: dict) -> dict:
     cfg = dict(architectures=["Qwen3ForCausalLM"], model_type="qwen3", max_position_embeddings=40960,
                rms_norm_eps=1e-6, rope_theta=1000000, hidden_act="silu", attention_bias=False,
                torch_dtype="bfloat16", bos_token_id=0, eos_token_id=1)
+    if is_moe(dims):
+        cfg.update(architectures=["Qwen3MoeForCausalLM"], model_type="qwen3_moe", decoder_sparse_step=1, mlp_only_layers=[],
+                   norm_topk_prob=True)
     cfg.update(dims)
     return cfg
 
@@ -53,10 +76,22 @@ def weight_shapes(d: dict) -> dict[str, tuple]:
         shapes.update({
             p + "self_attn.q_proj.weight": (hq * D, H), p + "self_attn.k_proj.weight": (hkv * D, H),
             p + "self_attn.v_proj.weight": (hkv * D, H), p + "self_attn.o_proj.weight": (H, hq * D),
-            p + "self_attn.q_norm.weight": (D,), p + "self_attn.k_norm.weight": (D,),
-            p + "mlp.gate_proj.weight": (I, H), p + "mlp.up_proj.weight": (I, H), p + "mlp.down_proj.weight": (H, I),
-            p + "input_layernorm.weight": (H,), p + "post_attention_layernorm.weight": (H,)})
+            p + "self_attn.q_norm.weight": (D,), p + "self_attn.k_norm.weight": (D,)})
+        if is_moe(d):                   # the Hub's per-expert names (Qwen3MoeSparseMoeBlock)
+            E, Ie = d["num_experts"], d["moe_intermediate_size"]
+            shapes[p + "mlp.gate.weight"] = (E, H)
+            for e in range(E):
+                q = f"{p}mlp.experts.{e}."
+                shapes.update({q + "gate_proj.weight": (Ie, H), q + "up_proj.weight": (Ie, H), q + "down_proj.weight": (H, Ie)})
+        else:                           # (this order is the order of random_weights' draws)
+            shapes.update({p + "mlp.gate_proj.weight": (I, H), p + "mlp.up_proj.weight": (I, H), p + "mlp.down_proj.weight": (H, I)})
+        shapes.update({p + "input_layernorm.weight": (H,), p + "post_attention_layernorm.weight": (H,)})
     return shapes
+
+
+def weight_std(name: str, shape: tuple, init_std: float = 0.02) -> float:
+    """Standard deviation of a matrix's random draw: ROUTER_LOGIT_STD / sqrt(hidden) for a MoE router, else init_std."""
+    return ROUTER_LOGIT_STD / shape[1] ** 0.5 if name.endswith(".mlp.gate.weight") else init_std
 
 
 def random_weights(dims: dict, seed: int = 0, init_std: float = 0.02) -> dict[str, torch.Tensor]:
@@ -66,7 +101,7 @@ def random_weights(dims: dict, seed: int = 0, init_std: float = 0.02) -> dict[st
         if len(shape) == 1:
             w = 1.0 + 0.1 * torch.randn(shape, generator=gen)
         else:
-            w = init_std * torch.randn(shape, generator=gen)
+            w = weight_std(name, shape, init_std) * torch.randn(shape, generator=gen)
         out[name] = w.to(torch.bfloat16)
     return out
 
@@ -115,6 +150,8 @@ def make_model_dir(path: str, preset: str | dict = "qwen3-0.6b", seed: int = 0, 
     stamp = os.path.join(path, ".synthetic.json")
     want = dict(dims=dims, seed=seed, init_std=init_std, weights=weights, tokenizer=tokenizer, v=2)
     if fp8:
+        if is_moe(dims):
+            raise NotImplementedError("FP8 mixture-of-experts checkpoints are not supported")
         want["fp8"] = True
     if os.path.exists(stamp):
         with open(stamp) as f:
